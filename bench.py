@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the per-ray rendering hot path (BASELINE.json metric: rays/s, fwd+bwd, NeRF-Synthetic-lego shape).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2|C3|C4]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2|C3|C4] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Headline (`value`, `e2e`, `roofline`): config C2 = nerf-blender HashGrid L16/F2/T2^19 + FullyFused-64 fields, 8192 rays per GPU.
@@ -18,6 +18,9 @@ At N = 1 the same JSON line also carries
     the CPU oracle's marching / compositing, fwd+bwd on the host cores; `cpu_baseline_secondary`: the fp32 CPU port of C2 itself.
 `--impl reference` times the CPU port of the headline config on the host cores at the SAME rays per step it reports.
 Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for every field.
+`--dump-outputs DIR` (rank 0) writes what the timed path computed in its last timed step as DIR/<name>.npy: the loss, the per-ray
+outputs of the captured step (per-sample outputs: the valid rows in packed order) and every parameter gradient (float32; integer outputs as float64; tensors above 2^20 entries as a fixed
+seeded sample of 2^20 of them).  Inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -46,7 +49,41 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'fallback (H100 SXM data sheet: 3.35 TB/s HBM3)'
+
+
+DUMP_MAX = 1 << 20   # entries kept per dumped tensor (a seeded sample above that)
+DUMP_BUDGET = 64 << 20   # bytes of all dumped arrays together
+
+
+def dump_outputs(path, loss, out, model):
+    """loss, the step's output dict and the parameter gradients -> path/<name>.npy (float32, integers as float64)."""
+    os.makedirs(path, exist_ok=True)
+    if 'loose_pos' in out:
+        # static NeRF training output: capacity-length buffers with the first num_samples rows valid, and `weights` in the loose layout
+        # whose row placement follows the marcher's atomic allocation.  Dump the valid rows in packed order, which does not vary.
+        k = int(out['num_samples_dev'])
+        pos = out['loose_pos'][:k]
+        out = {key: v for key, v in out.items() if key not in ('loose_pos', 'offsets_loose')}
+        out['weights'] = out['weights'][pos]
+        for key in ('t_starts', 't_ends', 'ray_indices'):
+            out[key] = out[key][:k]
+    arrays = {'loss': loss}
+    arrays.update({f'out.{k}': v for k, v in out.items() if torch.is_tensor(v)})
+    arrays.update({f'grad.{n}': p.grad for n, p in model.named_parameters() if p.grad is not None})
+    host = {}
+    for name, t in arrays.items():
+        a = t.detach().reshape(-1).cpu()
+        a = a.double() if not (a.is_floating_point() or a.is_complex()) else a.float()
+        if a.numel() > DUMP_MAX:
+            idx = torch.from_numpy(np.sort(np.random.default_rng(0).choice(a.numel(), DUMP_MAX, replace=False)))
+            a = a[idx]
+        host[name] = a.numpy()
+    total = sum(a.nbytes for a in host.values())
+    if total > DUMP_BUDGET:
+        raise SystemExit(f'bench.py --dump-outputs: {total} bytes of outputs exceed the {DUMP_BUDGET}-byte budget')
+    for name, a in host.items():
+        np.save(os.path.join(path, name + '.npy'), a)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -249,7 +286,7 @@ def masked_smooth_l1(comp_rgb, target, valid):
     return per.sum() / (m.sum() * 3.0).clamp(min=1.0)
 
 
-def neus_config(name, dev, steps, warmup, flush, peak, peak_src):
+def neus_config(name, dev, steps, warmup, flush, peak, peak_src, dump=None):
     """BASELINE.json config 3 (neus-blender with mask, 8192 rays; static-shape step = one CUDA graph) or config 4 (neus-dtu with learned
     background, 4096 rays; eager: the background pass has host-sized outputs) on one GPU: fwd + the reference's loss terms
     (systems/neus.py:98-121 as nsr_b200.losses.neus_losses) + bwd.  Returns a sub-line: rays/s (median of per-step CUDA events, L2
@@ -304,6 +341,7 @@ def neus_config(name, dev, steps, warmup, flush, peak, peak_src):
             loss.backward()
             step.last = out
             return loss
+    last_loss = None
     for i in range(warmup):
         step(rays_dev[i % pool], tgt_dev[i % pool], msk_dev[i % pool])
     torch.cuda.synchronize()
@@ -314,11 +352,13 @@ def neus_config(name, dev, steps, warmup, flush, peak, peak_src):
         flush.fill_(float(i))
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        step(rays_dev[j], tgt_dev[j], msk_dev[j])
+        last_loss = step(rays_dev[j], tgt_dev[j], msk_dev[j])
         e1.record()
         evs.append((e0, e1))
     torch.cuda.synchronize()
     launches = lib.launches
+    if dump is not None:
+        dump_outputs(dump, last_loss, gs.out if graphed else step.last, m)
     per = [a.elapsed_time(b) for a, b in evs]
     host = []
     for i in range(steps):
@@ -402,7 +442,7 @@ def neus_arm(args):
     peak, peak_src = peaks()
     sampler = ClockSampler(0)
     sampler.start()
-    sub = neus_config(args.config, dev, args.steps, max(3, args.warmup), flush, peak, peak_src)
+    sub = neus_config(args.config, dev, args.steps, max(3, args.warmup), flush, peak, peak_src, dump=args.dump_outputs)
     clocks = sampler.stop()
     line = dict(sub)
     line.update({'n_gpus': 1, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'data': 'synthetic', 'clocks': clocks})
@@ -440,7 +480,7 @@ def gpu_arm(args):
     tgt_dev = [t.to(dev) for t in tgt_np]
     rays_pin = [torch.from_numpy(r).pin_memory() for r in rays_np]
     tgt_pin = [t.pin_memory() for t in tgt_np]
-    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)  # > 50 MB L2
 
     from nsr_b200.losses import nerf_rgb_loss
 
@@ -528,6 +568,8 @@ def gpu_arm(args):
     per_step = timed(args.steps, e2e=False)
     barrier()
     launches = lib.launches
+    if args.dump_outputs and rank == 0:   # the static buffers of the graph still hold the last timed step
+        dump_outputs(args.dump_outputs, gstep.loss, gstep.out, model)
     # ---- end-to-end: pinned host buffers in, loss out, same K steps
     barrier()
     per_step_e2e = timed(args.steps, e2e=True)
@@ -637,29 +679,6 @@ def gpu_arm(args):
                  'algorithmic_bytes': opt_bytes, 'achieved_GBps': opt_bytes / (opt_ms * 1e-3) / 1e9,
                  'frac_of_hbm_peak': opt_bytes / (opt_ms * 1e-3) / 1e9 / peak, 'all_tensors_ms': opt_ms_all,
                  'train_step_ms_with_optimizer': ms_step + opt_ms_all}
-    # DRAM traffic of the dominant kernel from the committed ncu capture (per launch, same workload): far BELOW the algorithmic bytes
-    # because the table and its gradient are L2 resident
-    ncu_info = {}
-    try:
-        prof = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles')
-        name = 'r2_ncu_traffic.json' if os.path.exists(os.path.join(prof, 'r2_ncu_traffic.json')) else 'r1_ncu_traffic.json'
-        with open(os.path.join(prof, name)) as fh:
-            ncu_info = json.load(fh)
-    except (OSError, ValueError):
-        pass
-    if roofline is not None and dom in ncu_info:
-        roofline['traffic'] = ncu_info[dom].get('dram_bytes_per_launch')
-        roofline['traffic_source'] = ncu_info.get('source')
-    if roofline is not None and dom in ('nsr_nerf_field_bwd', 'nsr_nerf_field_bwd_tc') and dom in ncu_info:
-        # the table (25 MB fp16) and its gradient (50 MB fp32) live in the 126 MB L2: the kernel's real ceiling is the L2 atomic unit.
-        # ~80 REDs (8-byte red.global.add.v2.f32) per kept sample after run merging = ncu RED sectors / K
-        # (profiles/r1_ncu_traffic.json); 140 G RED/s = scatter-only micro-benchmark at full occupancy
-        # (profiles/r1_gather_scatter_microbench.md).
-        info = ncu_info.get(dom, {})
-        reds = (info['red_sectors_per_launch'] / info['kept_samples'] if 'red_sectors_per_launch' in info else 79.2) * k1
-        roofline['secondary'] = {'bound': 'l2_red', 'unit': 'G RED/s', 'achieved': reds / (kern[dom]['ms'] * 1e-3) / 1e9, 'peak': 140.0,
-                                 'frac': reds / (kern[dom]['ms'] * 1e-3) / 1e9 / 140.0,
-                                 'source': 'REDs/sample from ncu (profiles/r1_ncu_traffic.json); peak = measured scatter-only floor (profiles/r1_gather_scatter_microbench.md)'}
     cpu = time_cpu(4, 1, n_rays=CPU_SAMPLE_RAYS) if world == 1 else None   # ~5 s of CPU work: the C2 port (secondary)
     cpu_c1 = time_cpu_c1(4, 1) if world == 1 else None                       # ~10-15 s: BASELINE.json config 1 (primary)
     extra = {}
@@ -719,8 +738,12 @@ def main():
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--config', default='C2', choices=['C2', 'C3', 'C4'], help='headline config (C3 / C4: single GPU)')
     ap.add_argument('--no-extra', action='store_true', help='skip the C3 / C4 sub-lines of the default run')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help="write the last timed step's loss, outputs and parameter gradients to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == 'reference':
+        if args.dump_outputs:
+            ap.error('--dump-outputs applies to the GPU path only (--impl ours)')
         reference_arm(args)
     elif args.config == 'C2':
         gpu_arm(args)

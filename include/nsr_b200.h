@@ -1,4 +1,4 @@
-/* nsr_b200 -- C ABI of the B200-native per-ray rendering hot path (drop-in for the tiny-cuda-nn +
+/* nsr_b200 -- C ABI of the H100 (sm_90a) per-ray rendering hot path (drop-in for the tiny-cuda-nn +
  * nerfacc 0.3.3 calls made by bennyguo/instant-nsr-pl's models/).
  *
  * Conventions (SURVEY.md §8b):
@@ -138,9 +138,9 @@ int nsr_mlp_vanilla_fwd(const nsr_mlp_t* m, const void* x_h, const void* weights
 int nsr_mlp_vanilla_bwd(const nsr_mlp_t* m, const void* x_h, const void* weights_h, const float* bias, const float* dy,
                         float* grad_weights, float* grad_bias, float* dx, float loss_scale, const float* amax, int64_t n, void* stream);
 
-/* tcgen05 / TMEM version of nsr_mlp_fwd (same tensors): 128-row CTA tiles, operands in the canonical K-major smem layout,
- * accumulators in tensor memory, tcgen05.ld epilogue.  variant bit 0 = swap LBO/SBO in the smem descriptors (bring-up switch);
- * status: device int (may be NULL), set to 1 if an mbarrier wait timed out. */
+/* Warpgroup-MMA (wgmma) version of nsr_mlp_fwd (same tensors): 128-row CTA tiles, operands in the canonical K-major smem layout,
+ * fp32 accumulators in registers.  variant bit 0 = swap LBO/SBO in the smem descriptors (a layout check: wrong results);
+ * status: accepted for ABI compatibility, never written. */
 int nsr_mlp_fwd_tc(const nsr_mlp_t* m, const void* x_h, const void* params_h, void* out_h, int64_t n, int variant, int* status, void* stream);
 
 /* ---- marching / compositing (nerfacc 0.3.3 surface) ----------------------------------------- */
@@ -243,9 +243,9 @@ int nsr_nerf_field_bwd(const nsr_nerf_t* f, const float* rays, const int32_t* ra
  * coarse levels are summed across the warp before one lane issues the REDs, and x-adjacent corners that are neighbours in memory
  * leave as one 16-byte RED (autograd of tcnn's HashGrid, models/geometry.py:122-130).  Same results as nsr_nerf_field_bwd up to the fp16
  * rounding of d(encoding) and the summation order. */
-/* Blackwell-native form of the same backward (csrc/nerf_bwd_tc.cu): tcgen05.mma with the accumulators in tensor memory, tile inputs
- * staged by cp.async.bulk (TMA) + mbarrier, warp-specialised producer / MMA issuer / epilogue / scatter roles, weight gradients kept in
- * TMEM for the whole kernel.  enc_tiles_h = nsr_pack_kept(..., enc_tiled = 1); xyzdir / d_sraw / d_rgb in packed row order; all four
+/* Hopper tensor-core form of the same backward (csrc/nerf_bwd_tc.cu): wgmma.mma_async from shared memory, tile inputs staged by
+ * cp.async.bulk (TMA) + mbarrier, warp-specialised GEMM-chain / scatter roles, weight gradients accumulated in shared memory for the
+ * whole kernel.  enc_tiles_h = nsr_pack_kept(..., enc_tiled = 1); xyzdir / d_sraw / d_rgb in packed row order; all four
  * buffers readable up to the end of the last 128-row tile.  status (device int, may be NULL): non-zero if a barrier wait timed out. */
 int nsr_nerf_field_bwd_tc(const nsr_nerf_t* f, const void* enc_tiles_h, const void* dparams_h, const void* cparams_h, const float* d_sraw,
                           const float* d_rgb, float* grad_dparams, float* grad_cparams, float loss_scale, const float* amax, int64_t k,

@@ -1,8 +1,8 @@
-"""In-tree build of libnsr_b200.so (plain nvcc, sm_100a only, no torch headers).
+"""In-tree build of libnsr_b200.so (plain nvcc, sm_90a only, no torch headers).
 
     python instant-nsr-pl_b200/build.py [--force] [--verbose]
 
-The .so lands next to this file and travels to the GPU box with the repo snapshot.
+The .so lands next to this file, so the package imports straight from the source tree.
 """
 import os
 import subprocess
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(HERE, 'build')
 LIB = os.path.join(HERE, 'libnsr_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 COMMON = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '-Xcompiler', '-O3']
 # files whose float arithmetic must match the numpy oracle op-for-op (no implicit fma contraction)
 NO_FMAD = {'march.cu'}

@@ -45,13 +45,13 @@ def to_primitive(c):
     return c
 
 
-# kernel paths seen green (parity + timing) on a B200: on by default, NSR_DISABLE=name[,name] switches one off again
-VALIDATED = {'mlp_vanilla', 'radiance_vanilla', 'pack_scan'}   # round 2: profiles/r2_gputest_first.log
+# kernel paths seen green in the GPU suite: on by default, NSR_DISABLE=name[,name] switches one off again
+VALIDATED = {'mlp_vanilla', 'radiance_vanilla', 'pack_scan'}
 
 
 def experimental(name):
     """True when the kernel path ``name`` is switched on.  Paths in VALIDATED are on unless NSR_DISABLE lists them; any other name is a
-    path that has not run on a B200 yet and stays off unless the environment asks for it: NSR_EXPERIMENTAL=1 (all) or a comma-separated
+    path that has not passed the GPU suite yet and stays off unless the environment asks for it: NSR_EXPERIMENTAL=1 (all) or a comma-separated
     list of names."""
     import os
     if name in [x.strip() for x in os.environ.get('NSR_DISABLE', '').split(',') if x.strip()]:

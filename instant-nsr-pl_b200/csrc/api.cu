@@ -11,13 +11,16 @@ void nsr_set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+// launch-shape fallback when the device query fails: the SM count of an H100 SXM (the launch itself then reports the error)
+constexpr int kFallbackSms = 132;
+
 int nsr_sm_count() {
   static thread_local int cached_dev = -1, cached = 0;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return kFallbackSms;
   if (dev != cached_dev) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kFallbackSms;
     cached = n;
     cached_dev = dev;
   }

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the nsr_b200 kernels (sm_100a only).
+// Shared device/host helpers for the nsr_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -70,7 +70,7 @@ __device__ __forceinline__ void nsr_corner_indices(const LevelInfo& li, uint32_t
       uint32_t i = b + (c & 1) + ((c >> 1) & 1) * r + ((c >> 2) & 1) * r2;
       // i % size without the integer division: a dense level has res^3 <= size, so an in-range cell gives i < 2 size (res >= 2) and
       // i % size == i - (i >= size) * size; anything else (a NaN / out-of-box position) is clamped first and stays in bounds.  The
-      // division cost 11 % of the per-ray forward kernel's instructions (ncu, round 2).
+      // integer division was a visible share of the per-ray forward kernel's instructions.
       i = min(i, 2u * li.size - 1u);          // (branch-free: clamp, then one conditional subtract)
       i -= i >= li.size ? li.size : 0u;
       idx[c] = i + li.offset;

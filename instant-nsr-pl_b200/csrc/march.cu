@@ -5,7 +5,7 @@
 // explicit __fmaf_rn) in exactly the order oracle/march.py performs it, so that the emitted sample
 // SET is bit-identical to the oracle's.
 //
-// B200 design: instead of nerfacc's one-thread-per-ray serial march (<= ~1024 dependent iterations,
+// Design: instead of nerfacc's one-thread-per-ray serial march (<= ~1024 dependent iterations,
 // long-tail divergence), the cone_angle == 0 case tests the step lattice in parallel -- one warp per
 // ray, 32 lattice points per iteration, ballot + popc compaction -- against a packed BITfield
 // (128^3 bits = 256 KB, L1/L2 resident; nerfacc reads 2 MB of bools).  Two passes (count, write)

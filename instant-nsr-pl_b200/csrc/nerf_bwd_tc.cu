@@ -1,27 +1,27 @@
-// Blackwell-native form of the fused NeRF backward (autograd of VolumeRadiance + VolumeDensity + HashGrid, models/texture.py:23-30,
-// models/geometry.py:122-130; tcnn: FullyFusedMLP backward + grid backward): tcgen05.mma with accumulators in tensor memory, tile
-// inputs staged by the TMA engine (cp.async.bulk + mbarrier), warp-specialised roles.
+// Hopper tensor-core form of the fused NeRF backward (autograd of VolumeRadiance + VolumeDensity + HashGrid, models/texture.py:23-30,
+// models/geometry.py:122-130; tcnn: FullyFusedMLP backward + grid backward): warpgroup MMAs (wgmma.mma_async, sm_90a) with both
+// operands in shared memory, tile inputs staged by the TMA engine (cp.async.bulk + mbarrier), warp-specialised roles.
 //
-// One CTA = 16 warps, two CTAs per SM, persistent over 128-row tiles of kept samples (packed, ray-major order):
-//   warp 0      producer: one lane issues four cp.async.bulk copies per tile (encodings in the canonical UMMA tile layout written by
-//               nsr_pack_kept, position + direction, d sigma_raw, d rgb = 13 KB) into a two-stage ring; the warp also owns the TMEM allocation
-//   warp 1      MMA issuer: one lane walks the ten dependent GEMMs of a tile -- five forward-recompute layers, five dgrad layers -- and
-//               issues, next to each dgrad, the weight-gradient GEMM of that layer (M = 64, K = 128 samples) whose accumulator stays in
-//               TMEM for the whole kernel; every group ends in tcgen05.commit -> mbarrier
-//   warps 4-7   epilogue: thread = row; tcgen05.ld the accumulator row, activation / ReLU mask (from the fp16 activations the tile holds) /
-//               incoming-gradient injection, re-pack to fp16 and store the row into the next GEMM's A operand in the canonical K-major
-//               layout (which, read through an MN-major descriptor, is also the weight-gradient GEMM's operand: no transposes anywhere)
-//   warps 8-15  scatter, two groups that alternate tiles: thread = row; pull d(encoding) (32 fp32 columns) out of TMEM, then per level
-//               corner weights, warp-wide merging of runs that share a cell, paired 16-byte REDs into the fp32 gradient table
-// The GEMM chain of tile t+1 runs while the scatter warps are still issuing the REDs of tiles t and t-1; the REDs come from 16 light
-// warps per SM instead of the 8 register-heavy MMA warps of nerf_bwd_kernel (csrc/nerf_fused_bwd.cu), which was its bound.
+// One CTA = 16 warps, one CTA per SM, persistent over 128-row tiles of kept samples (packed, ray-major order):
+//   warps 0-7   two chain warpgroups; warpgroup c owns rows [64 c, 64 c + 64) of every tile and walks the ten dependent GEMMs of its
+//               half -- five forward-recompute layers, five dgrad layers -- plus, next to each dgrad, the weight-gradient GEMM of that
+//               layer (M = 64, K = the 64 samples).  Accumulators are registers; the epilogue (activation / ReLU mask from the fp16
+//               activations the tile holds / incoming-gradient injection) re-packs to fp16 and stores into the next GEMM's A operand in
+//               the canonical K-major layout, which read through an MN-major descriptor is also the weight-gradient GEMM's operand: no
+//               transposes anywhere.  Weight-gradient partials are added into a shared fp32 accumulator, flushed once at the end.
+//               The last GEMM's d(encoding) goes to a two-slot shared buffer for the scatter warps.
+//   warps 8-15  scatter, two groups that alternate tiles and own one stage of the two-stage input ring each: thread = row; read
+//               d(encoding) (16 fp16 pairs), then per level corner weights, warp-wide merging of runs that share a cell, paired 16-byte
+//               REDs into the fp32 gradient table.  Once every reader is done with the group's stage, one lane refills it with the
+//               tile after next: four cp.async.bulk copies (encodings in the canonical tile layout written by nsr_pack_kept, position +
+//               direction, d sigma_raw, d rgb = 13 KB).  (A separate producer warp would cost the chain 32 registers per thread.)
+// The GEMM chain of tile t+1 runs while the scatter warps are still issuing the REDs of tiles t and t-1.
 //
-// Shared memory (110 KB): weights of both networks, canonical [out][in] (one copy serves the forward GEMMs as K-major B and the dgrad
+// Shared memory (170 KB): weights of both networks, canonical [out][in] (one copy serves the forward GEMMs as K-major B and the dgrad
 // GEMMs as MN-major B); activation tiles H1, CI, G1, G2 which the dgrad epilogues overwrite in place with dH1, dG1, dG2; dC3, dO;
-// two stages of tile inputs.  Tensor memory (256 columns): 64 chain accumulator + 32 d(encoding) + 160 weight gradients.
-#include <stdio.h>
-#include <stdlib.h>
+// two stages of tile inputs; two d(encoding) slots; the weight-gradient accumulator.
 #include "nerf_fused.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -46,54 +46,21 @@ constexpr int A_END = A_DO + kRows * 16 * 2;
 constexpr int S_X0 = 0, S_XYZ = S_X0 + kRows * 32 * 2, S_DS = S_XYZ + kRows * 6 * 4, S_DRGB = S_DS + kRows * 4, S_STAGE = S_DRGB + kRows * 3 * 4;
 constexpr int kStageBytes = S_STAGE;  // 13312
 constexpr int STAGES = A_END;
-constexpr int BARS = STAGES + 2 * kStageBytes;
+// d(encoding) slots: [128 rows][16 levels] fp16 pairs, rows padded to 20 words (conflict-free 16-byte reads by the scatter warps)
+constexpr int DE_STRIDE = 20;
+constexpr int DE = STAGES + 2 * kStageBytes;
+constexpr int kDeBytes = kRows * DE_STRIDE * 4;
+// weight-gradient accumulator: one fp32 slot per (accumulator register, chain thread): both warpgroups add into the same slots
+constexpr int G_DW1 = 0, G_DW2 = G_DW1 + 16, G_CW1 = G_DW2 + 8, G_CW2 = G_CW1 + 16, G_CW3 = G_CW2 + 32, G_SLOTS = G_CW3 + 8;  // 80
+constexpr int WACC = DE + 2 * kDeBytes;
+constexpr int BARS = WACC + G_SLOTS * 128 * 4;
 constexpr int kSmemBytes = BARS + 128;
-static_assert(kStageBytes % 16 == 0 && STAGES % 128 == 0, "alignment");
-
-// ---- tensor-memory map (columns) ----------------------------------------------------------------------------------------------
-constexpr uint32_t T_ACC = 0, T_DE = 64, T_WDW1 = 96, T_WDW2 = 128, T_WCW1 = 144, T_WCW2 = 176, T_WCW3 = 240, T_COLS = 256;
+static_assert(kStageBytes % 16 == 0 && STAGES % 128 == 0 && DE % 16 == 0 && WACC % 16 == 0, "alignment");
+static_assert(kSmemBytes <= 227 * 1024, "shared memory");
 
 // barrier slots (8 bytes each)
-enum { B_FULL0 = 0, B_FULL1, B_EMPTY0, B_EMPTY1, B_MMA, B_EPI, B_DEFULL0, B_DEFULL1, B_DEEMPTY0, B_DEEMPTY1, B_WG, B_COUNT };
+enum { B_FULL0 = 0, B_FULL1, B_EMPTY0, B_EMPTY1, B_DEFULL0, B_DEFULL1, B_DEEMPTY0, B_DEEMPTY1, B_COUNT };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// canonical (no-swizzle) UMMA layout of a [rows][K] fp16 tile: 8 x 16-byte core matrices, K chunks 128 B apart, 8-row groups (K/8)*128 B apart
-__device__ __forceinline__ int canon_off(int row, int k, int K) { return ((row >> 3) * (K >> 3) + (k >> 3)) * 128 + (row & 7) * 16 + (k & 7) * 2; }
-
-// Shared-memory matrix descriptors (no swizzle, sm_100 version bit 46), written as  lo = (address >> 4) + constant, hi = constant  so that the
-// issuing thread needs ONE add per operand behind a barrier wait (the first version re-derived mask / shift / or chains from the byte address
-// for every MMA: ~40 dependent uniform-datapath instructions per GEMM group, 400-1000 cycles on the critical path of every chain step).
-//   K-major  [rows][K] tile (rows = M/N index, K contiguous): LBO = 128 B between the two 8-wide K chunks of one MMA, SBO = (K/8)*128 B between
-//            8-row groups; MMA kk starts 256 B further            => lo = b16 + (8 << 16) + 16 kk,      hi = K | 0x4000
-//   MN-major the same physical tile [k rows][C cols] read with M/N along the columns: SBO = 128 B between 8-column chunks, LBO = (C/8)*128 B
-//            between 8-row k groups; MMA kk starts 2 LBO further  => lo = b16 + (C << 16) + 2 C kk,     hi = 8 | 0x4000
-__device__ __forceinline__ uint32_t dk_lo(uint32_t b16, int kk) { return b16 + (8u << 16) + 16u * (uint32_t)kk; }
-__device__ __forceinline__ uint32_t dk_hi(int K) { return (uint32_t)K | 0x4000u; }
-__device__ __forceinline__ uint32_t dm_lo(uint32_t b16, int C, int kk) { return b16 + ((uint32_t)C << 16) + 2u * (uint32_t)C * (uint32_t)kk; }
-__device__ __forceinline__ uint32_t dm_hi() { return 8u | 0x4000u; }
-// kind::f16: D f32 (1 @4), A = B = f16, a_major @15, b_major @16 (1 = MN-major), N>>3 @17, M>>4 @24
-__device__ __forceinline__ uint32_t make_idesc(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma(uint32_t d_tmem, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc, uint32_t accumulate,
-                                     int skip = 0) {
-  if (skip) return;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
@@ -104,8 +71,7 @@ __device__ __forceinline__ void tma_bulk(uint32_t dst, const void* src, uint32_t
                : "memory");
 }
 // bounded wait: a barrier that is never signalled (a bug) sets *status and traps instead of hanging the GPU
-// acc (development, NSR_TC_TRACE): cycles spent in the wait are added to acc[code * 16]
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* status, int code, long long* acc = nullptr) {
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* status, int code) {
   const long long t0 = clock64();
   for (;;) {
     uint32_t ok;
@@ -118,46 +84,32 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* st
         : "=r"(ok)
         : "r"(bar), "r"(parity)
         : "memory");
-    if (ok) {
-      if (acc != nullptr) atomicAdd(reinterpret_cast<unsigned long long*>(acc + code * 16), (unsigned long long)(clock64() - t0));
-      return;
-    }
+    if (ok) return;
     if (clock64() - t0 > 4000000000ll) {
       if (status) atomicExch(status, code);
       __trap();
     }
   }
 }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void proxy_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// barrier of the 128 threads of chain warpgroup c (ids 1, 2); id 3 joins both chain warpgroups
+__device__ __forceinline__ void wg_bar(int c) { asm volatile("bar.sync %0, 128;" ::"r"(1 + c) : "memory"); }
+__device__ __forceinline__ void chain_bar() { asm volatile("bar.sync 3, 256;" ::: "memory"); }
 
 // row-major [rows][K] fp16 matrix (global) -> canonical smem tile
 __device__ __forceinline__ void stage_canonical(uint8_t* dst, const __half* __restrict__ src, int rows, int K) {
   const int vec_per_row = K / 8;
   for (int i = threadIdx.x; i < rows * vec_per_row; i += blockDim.x) {
     const int r = i / vec_per_row, kc = i % vec_per_row;
-    *reinterpret_cast<uint4*>(dst + canon_off(r, kc * 8, K)) = __ldg(reinterpret_cast<const uint4*>(src + (size_t)r * K) + kc);
+    *reinterpret_cast<uint4*>(dst + nsr_canon_off(r, kc * 8, K)) = __ldg(reinterpret_cast<const uint4*>(src + (size_t)r * K) + kc);
   }
+}
+
+// descriptors of a canonical tile at byte address `addr`, k16 step kk:
+//   K-major  [rows][K]: LBO = 128 B (the two 8-wide K chunks), SBO = (K/8)*128 B (8-row groups); step kk starts 256 B further
+//   MN-major [k rows][C] read with M / N along C: SBO = 128 B (8-column chunks), LBO = (C/8)*128 B (8-row k groups); step kk = 2 LBO
+__device__ __forceinline__ uint64_t dk(uint32_t addr, int K, int kk) { return nsr_wg_desc(addr + 256u * (uint32_t)kk, 128u, (uint32_t)(K / 8) * 128u); }
+__device__ __forceinline__ uint64_t dm(uint32_t addr, int C, int kk) {
+  return nsr_wg_desc(addr + 2u * (uint32_t)(C / 8) * 128u * (uint32_t)kk, (uint32_t)(C / 8) * 128u, 128u);
 }
 
 struct TcArgs {
@@ -174,77 +126,40 @@ struct TcArgs {
   int64_t n_cap;
   float loss_scale;
   int* status;
-  long long* trace;  // NSR_TC_TRACE: [3 CTAs][16 wait codes][16 warps] cycle counters (row 0: warp lifetime); else NULL
-  int dbg;  // development A/B switches (NSR_TC_DEBUG): 1 = no REDs, 2 = scatter warps do not wait for the chain, 4 = scatter warps idle,
-            // 128 = scatter uses a synthetic non-zero d(encoding) (with 2 / 8: the scatter's own speed at the full RED count),
-            // 32 = hidden-layer epilogues do nothing (no tcgen05.ld, no st.shared), 64 = no tcgen05.mma (commits only): timing experiments,
-            // 16 = epilogue skips fence.proxy.async (timing experiment only: results undefined),
-            // 8 = no GEMM chain (MMA / epilogue warps only keep the stage barriers moving): with 2 the scatter runs alone
 };
 
-// wait for the tcgen05.ld results; the registers are in/out operands so that no use of them can be scheduled in front of the wait
-__device__ __forceinline__ void tmem_ld_wait16(uint32_t (&v)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]), "+r"(v[8]), "+r"(v[9]), "+r"(v[10]),
-                 "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15])
-               :
-               : "memory");
-}
-
-// 16 accumulator columns [c0, c0 + 16) of the thread's row -> two 16-byte chunks of the canonical K = 64 tile
+// epilogue of a 64-wide hidden layer from the accumulator fragment into a canonical K = 64 tile (rows rr[0], rr[1])
 //   MODE 0: ReLU on the packed pair (round, then max with +0: same value as rounding max(x, 0))
-//   MODE 1: dgrad through ReLU, IN PLACE: the tile still holds this layer's fp16 activations; a gradient survives where its activation
-//           is > 0 (__hgt2_mask: ordered compare, a NaN activation masks like the fp32 test did)
+//   MODE 1: dgrad through ReLU, IN PLACE: the tile still holds this layer's fp16 activations (written by this same thread in the
+//           forward epilogue); a gradient survives where its activation is > 0 (__hgt2_mask: ordered compare, a NaN activation masks)
+// Rows past the end of the batch (keep = 0) are written as zeros.
 template <int MODE>
-__device__ __forceinline__ void epi_chunk16(const uint32_t (&v)[16], uint8_t* tile, int row, int c0, uint32_t keep) {
+__device__ __forceinline__ void epi64(const float (&d)[32], uint8_t* tile, const int (&rr)[2], const uint32_t (&keep)[2], int c0) {
   const __half2 zero = __float2half2_rn(0.f);
 #pragma unroll
-  for (int q = 0; q < 2; ++q) {
-    uint4* dst = reinterpret_cast<uint4*>(tile + canon_off(row, c0 + 8 * q, 64));
-    uint32_t pk[4];
-    uint4 act = make_uint4(0u, 0u, 0u, 0u);
-    if (MODE == 1) act = *dst;
-    const uint32_t am[4] = {act.x, act.y, act.z, act.w};
+  for (int j = 0; j < 8; ++j)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const __half2 h = __floats2half2_rn(__uint_as_float(v[8 * q + 2 * j]), __uint_as_float(v[8 * q + 2 * j + 1]));
+    for (int h = 0; h < 2; ++h) {
+      uint32_t* p = reinterpret_cast<uint32_t*>(tile + nsr_canon_off(rr[h], 8 * j + c0, 64));
+      const __half2 v = __floats2half2_rn(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
       if (MODE == 0) {
-        const __half2 r = __hmax2(h, zero);
-        pk[j] = *reinterpret_cast<const uint32_t*>(&r) & keep;
+        const __half2 r = __hmax2(v, zero);
+        *p = *reinterpret_cast<const uint32_t*>(&r) & keep[h];
       } else {
-        pk[j] = *reinterpret_cast<const uint32_t*>(&h) & __hgt2_mask(*reinterpret_cast<const __half2*>(&am[j]), zero) & keep;
+        const uint32_t act = *p;
+        *p = *reinterpret_cast<const uint32_t*>(&v) & __hgt2_mask(*reinterpret_cast<const __half2*>(&act), zero) & keep[h];
       }
     }
-    *dst = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-  }
 }
 
-// epilogue of a 64-wide hidden layer: ACC[row][0..63] -> fp16 row of a canonical K = 64 tile; ~25 instructions per 16 columns, the
-// tcgen05.ld of chunk i+1 in flight while chunk i is converted (the first version spent ~150 instructions per 16 columns on 64-bit ReLU
-// masks kept in registers).  The thread reads and rewrites only its own row, and every tensor-core read of the tile (the dgrad / wgrad
-// GEMMs of this step) has completed (commit -> B_MMA).  Rows past the end of the batch (live == false) are written as zeros.
-template <int MODE>
-__device__ __forceinline__ void epi_hidden(uint32_t lane_addr, uint8_t* tile, int row, bool live, int skip = 0) {
-  if (skip) return;
-  const uint32_t keep = live ? 0xFFFFFFFFu : 0u;
-  uint32_t va[16], vb[16];
-  tmem_ld16(lane_addr + T_ACC, va);
-  tmem_ld_wait16(va);
-  tmem_ld16(lane_addr + T_ACC + 16u, vb);
-  epi_chunk16<MODE>(va, tile, row, 0, keep);
-  tmem_ld_wait16(vb);
-  tmem_ld16(lane_addr + T_ACC + 32u, va);
-  epi_chunk16<MODE>(vb, tile, row, 16, keep);
-  tmem_ld_wait16(va);
-  tmem_ld16(lane_addr + T_ACC + 48u, vb);
-  epi_chunk16<MODE>(va, tile, row, 32, keep);
-  tmem_ld_wait16(vb);
-  epi_chunk16<MODE>(vb, tile, row, 48, keep);
+template <int R>
+__device__ __forceinline__ void wacc_add(float* wacc, int slot0, int t, const float (&w)[R]) {
+#pragma unroll
+  for (int r = 0; r < R; ++r) atomicAdd(wacc + (slot0 + r) * 128 + t, w[r]);
 }
 
-__global__ void __launch_bounds__(kThreads, 2) nerf_bwd_tc_kernel(const __grid_constant__ nsr_nerf_t P, const TcArgs a) {
+__global__ void __launch_bounds__(kThreads, 1) nerf_bwd_tc_kernel(const __grid_constant__ nsr_nerf_t P, const TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ uint32_t s_tmem;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int64_t n = a.n_dev ? min(*a.n_dev, a.n_cap) : a.n_cap;
   const int64_t n_tiles = (n + kRows - 1) / kRows;
@@ -254,26 +169,20 @@ __global__ void __launch_bounds__(kThreads, 2) nerf_bwd_tc_kernel(const __grid_c
     loss_scale = exp2f(fminf(fmaxf(floorf(log2f(256.f / amax)), -24.f), 60.f));
   }
   const float inv_scale = 1.f / loss_scale;
-  const uint32_t sbase = smem_u32(smem);
+  const uint32_t sbase = nsr_smem_u32(smem);
   const uint32_t bars = sbase + BARS;
   auto bar = [&](int i) { return bars + 8u * (uint32_t)i; };
+  float* wacc = reinterpret_cast<float*>(smem + WACC);
 
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 256;" ::"r"(smem_u32(&s_tmem)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (tid == 32) {
+  if (tid == 0) {
     mbar_init(bar(B_FULL0), 1);
     mbar_init(bar(B_FULL1), 1);
-    mbar_init(bar(B_EMPTY0), 9);  // MMA commit + 4 epilogue warps + 4 scatter warps
-    mbar_init(bar(B_EMPTY1), 9);
-    mbar_init(bar(B_MMA), 1);
-    mbar_init(bar(B_EPI), 4);
-    mbar_init(bar(B_DEFULL0), 1);
-    mbar_init(bar(B_DEFULL1), 1);
+    mbar_init(bar(B_EMPTY0), 12);  // 8 chain warps + 4 scatter warps
+    mbar_init(bar(B_EMPTY1), 12);
+    mbar_init(bar(B_DEFULL0), 8);
+    mbar_init(bar(B_DEFULL1), 8);
     mbar_init(bar(B_DEEMPTY0), 4);
     mbar_init(bar(B_DEEMPTY1), 4);
-    mbar_init(bar(B_WG), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   stage_canonical(smem + W_DW1, a.dparams, 64, 32);
@@ -281,355 +190,307 @@ __global__ void __launch_bounds__(kThreads, 2) nerf_bwd_tc_kernel(const __grid_c
   stage_canonical(smem + W_CW1, a.cparams, 64, 32);
   stage_canonical(smem + W_CW2, a.cparams + 64 * 32, 64, 64);
   stage_canonical(smem + W_CW3, a.cparams + 64 * 32 + 64 * 64, 16, 64);
-  proxy_fence();
-  tc_fence_before();
+  for (int i = tid; i < G_SLOTS * 128; i += kThreads) wacc[i] = 0.f;
+  nsr_proxy_fence();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
-  // development counters: three CTAs report, one row of 16 per wait code, one column per warp (lane 0 only); row 0 = the warp's lifetime
-  const int tsel = blockIdx.x == 0 ? 0 : ((int)blockIdx.x == (int)gridDim.x / 2 ? 1 : ((int)blockIdx.x == (int)gridDim.x - 1 ? 2 : -1));
-  long long* const acc = (a.trace != nullptr && tsel >= 0 && lane == 0) ? a.trace + tsel * 256 + warp : nullptr;
-  const long long t_begin = clock64();
   const int64_t my_tiles = n_tiles > (int64_t)blockIdx.x ? (n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
 
-  if (warp == 0) {
-    // ================================ producer ================================
-    if (lane == 0) {
-      for (int64_t it = 0; it < my_tiles; ++it) {
-        const int s = (int)(it & 1);
-        const int64_t tile = blockIdx.x + it * gridDim.x, row0 = tile * kRows;
-        mbar_wait(bar(B_EMPTY0 + s), (uint32_t)(((it >> 1) & 1) ^ 1), a.status, 1, acc);
-        const uint32_t dst = sbase + STAGES + (uint32_t)s * kStageBytes, fb = bar(B_FULL0 + s);
-        mbar_expect_tx(fb, kStageBytes);
-        tma_bulk(dst + S_X0, a.enc_tiles + tile * (kRows * 32 * 2), kRows * 32 * 2, fb);
-        tma_bulk(dst + S_XYZ, a.xyzdir + row0 * 6, kRows * 6 * 4, fb);
-        tma_bulk(dst + S_DS, a.d_sraw + row0, kRows * 4, fb);
-        tma_bulk(dst + S_DRGB, a.d_rgb + row0 * 3, kRows * 3 * 4, fb);
-      }
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ================================
-    // The whole warp walks the loop (converged: every lane waits on the barriers) and ONE elected lane issues each group: behind
-    // elect.sync the compiler emits the tcgen05 instructions straight from uniform registers.  (Issuing under `if (lane == 0)` made it wrap
-    // every UTCHMMA in an ELECT / BRA.U.ANY loop: ~55 cycles per MMA, 600-850 cycles per GEMM group in the first version's trace.)
-    uint32_t p_epi = 0;
-    const uint32_t sb16 = (sbase & 0x3FFFFu) >> 4;   // every tile offset is a multiple of 16 bytes: descriptors are sb16 + constants
-    const uint32_t w_dw1 = sb16 + W_DW1 / 16, w_dw2 = sb16 + W_DW2 / 16, w_cw1 = sb16 + W_CW1 / 16, w_cw2 = sb16 + W_CW2 / 16, w_cw3 = sb16 + W_CW3 / 16;
-    const uint32_t h1 = sb16 + A_H1 / 16, ci = sb16 + A_CI / 16, g1 = sb16 + A_G1 / 16, g2 = sb16 + A_G2 / 16, dc3 = sb16 + A_DC3 / 16, dO = sb16 + A_DO / 16;
-    const uint32_t i_fwd64 = make_idesc(128, 64, 0, 0), i_fwd16 = make_idesc(128, 16, 0, 0);
-    const uint32_t i_dg64 = make_idesc(128, 64, 0, 1), i_dg32 = make_idesc(128, 32, 0, 1), i_dg16 = make_idesc(128, 16, 0, 1);
-    const uint32_t i_wg64 = make_idesc(64, 64, 1, 1), i_wg32 = make_idesc(64, 32, 1, 1), i_wg16 = make_idesc(64, 16, 1, 1);
-    int tr_n = 1024;   // development: CTA 0, tiles 2..5: clock stamps of the hand-off loop (tools/tc_trace.py)
-    int64_t tr_it = 0;
-    auto stamp = [&]() {
-      if (a.trace != nullptr && blockIdx.x == 0 && lane == 0 && tr_it >= 2 && tr_n < 2048) a.trace[tr_n++] = clock64();
+  if (warp < 8) {
+    // ================================ chain warpgroups ================================
+    const int c = warp >> 2, t = tid & 127;
+    const int R0 = 64 * c;
+    // accumulator fragment of this thread: rows rr[0], rr[1] of the tile, columns 8 j + c0 (+1)
+    const int c0 = 2 * (lane & 3);
+    const int rr[2] = {R0 + 16 * (warp & 3) + (lane >> 2), R0 + 16 * (warp & 3) + (lane >> 2) + 8};
+    // operand addresses of this warpgroup's 64-row half (64 rows of a [128][K] canonical tile = K * 128 bytes)
+    const uint32_t h1 = sbase + A_H1 + c * 64 * 128, ci = sbase + A_CI + c * 32 * 128, g1 = sbase + A_G1 + c * 64 * 128;
+    const uint32_t g2 = sbase + A_G2 + c * 64 * 128, dc3 = sbase + A_DC3 + c * 16 * 128, dO = sbase + A_DO + c * 16 * 128;
+    const uint32_t w_dw1 = sbase + W_DW1, w_dw2 = sbase + W_DW2, w_cw1 = sbase + W_CW1, w_cw2 = sbase + W_CW2, w_cw3 = sbase + W_CW3;
+    // every GEMM step: make this warpgroup's epilogue stores visible to the tensor core, issue, wait; then a barrier so that no thread
+    // overwrites an operand tile in place before the whole warpgroup's MMAs have read it
+    auto begin = [&]() {
+      nsr_proxy_fence();
+      wg_bar(c);
+      nsr_wg_fence();
     };
-    auto wait_epi = [&]() {
-      stamp();   // previous group issued + committed
-      mbar_wait(bar(B_EPI), p_epi, a.status, 2, acc);
-      p_epi ^= 1u;
-      tc_fence_after();
-      stamp();   // operand tile ready
+    auto end = [&]() {
+      nsr_wg_commit();
+      nsr_wg_wait0();
+      wg_bar(c);
     };
     for (int64_t it = 0; it < my_tiles; ++it) {
       const int s = (int)(it & 1);
-      const uint32_t x0 = sb16 + (STAGES + S_X0) / 16 + (uint32_t)s * (kStageBytes / 16);
-      const uint32_t acc_first = it > 0 ? 1u : 0u;  // weight-gradient accumulators: overwrite on the CTA's first tile, then accumulate
-      tr_it = it;
-      mbar_wait(bar(B_FULL0 + s), (uint32_t)((it >> 1) & 1), a.status, 3, acc);
-      tc_fence_after();
-      if (a.dbg & 8) {
-        if (elect_one()) {
-          umma_commit(bar(B_DEFULL0 + s));
-          umma_commit(bar(B_EMPTY0 + s));
-        }
-        __syncwarp();
-        continue;
-      }
-      // 1: H1pre = X0 . DW1^T
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk) umma(tmem + T_ACC, dk_lo(x0, kk), dk_hi(32), dk_lo(w_dw1, kk), dk_hi(32), i_fwd64, kk > 0, a.dbg & 64);
-        umma_commit(bar(B_MMA));
-      }
-      __syncwarp();
-      // 2: Opre = H1 . DW2^T
-      wait_epi();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma(tmem + T_ACC, dk_lo(h1, kk), dk_hi(64), dk_lo(w_dw2, kk), dk_hi(64), i_fwd16, kk > 0, a.dbg & 64);
-        umma_commit(bar(B_MMA));
-      }
-      __syncwarp();
-      // 3: G1pre = [O | SH] . CW1^T
-      wait_epi();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk) umma(tmem + T_ACC, dk_lo(ci, kk), dk_hi(32), dk_lo(w_cw1, kk), dk_hi(32), i_fwd64, kk > 0, a.dbg & 64);
-        umma_commit(bar(B_MMA));
-      }
-      __syncwarp();
-      // 4: G2pre = G1 . CW2^T
-      wait_epi();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma(tmem + T_ACC, dk_lo(g1, kk), dk_hi(64), dk_lo(w_cw2, kk), dk_hi(64), i_fwd64, kk > 0, a.dbg & 64);
-        umma_commit(bar(B_MMA));
-      }
-      __syncwarp();
-      // 5: rgb_pre = G2 . CW3^T
-      wait_epi();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma(tmem + T_ACC, dk_lo(g2, kk), dk_hi(64), dk_lo(w_cw3, kk), dk_hi(64), i_fwd16, kk > 0, a.dbg & 64);
-        umma_commit(bar(B_MMA));
-      }
-      __syncwarp();
-      // 6: dG2pre = dC3 . CW3 ; dCW3^T += G2^T . dC3
-      wait_epi();
-      if (elect_one()) {
-        umma(tmem + T_ACC, dk_lo(dc3, 0), dk_hi(16), dm_lo(w_cw3, 64, 0), dm_hi(), i_dg64, 0u, a.dbg & 64);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) umma(tmem + T_WCW3, dm_lo(g2, 64, kk), dm_hi(), dm_lo(dc3, 16, kk), dm_hi(), i_wg16, kk > 0 ? 1u : acc_first, a.dbg & 64);
-        umma_commit(bar(B_MMA));
-      }
-      __syncwarp();
-      // 7: dG1pre = dG2 . CW2 ; dCW2 += dG2^T . G1
-      wait_epi();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma(tmem + T_ACC, dk_lo(g2, kk), dk_hi(64), dm_lo(w_cw2, 64, kk), dm_hi(), i_dg64, kk > 0, a.dbg & 64);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) umma(tmem + T_WCW2, dm_lo(g2, 64, kk), dm_hi(), dm_lo(g1, 64, kk), dm_hi(), i_wg64, kk > 0 ? 1u : acc_first, a.dbg & 64);
-        umma_commit(bar(B_MMA));
-      }
-      __syncwarp();
-      // 8: dOpre = dG1 . CW1[:, 0:16] ; dCW1 += dG1^T . CI
-      wait_epi();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma(tmem + T_ACC, dk_lo(g1, kk), dk_hi(64), dm_lo(w_cw1, 32, kk), dm_hi(), i_dg16, kk > 0, a.dbg & 64);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) umma(tmem + T_WCW1, dm_lo(g1, 64, kk), dm_hi(), dm_lo(ci, 32, kk), dm_hi(), i_wg32, kk > 0 ? 1u : acc_first, a.dbg & 64);
-        umma_commit(bar(B_MMA));
-      }
-      __syncwarp();
-      // 9: dH1pre = dO . DW2 ; dDW2^T += H1^T . dO
-      wait_epi();
-      if (elect_one()) {
-        umma(tmem + T_ACC, dk_lo(dO, 0), dk_hi(16), dm_lo(w_dw2, 64, 0), dm_hi(), i_dg64, 0u, a.dbg & 64);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) umma(tmem + T_WDW2, dm_lo(h1, 64, kk), dm_hi(), dm_lo(dO, 16, kk), dm_hi(), i_wg16, kk > 0 ? 1u : acc_first, a.dbg & 64);
-        umma_commit(bar(B_MMA));
-      }
-      __syncwarp();
-      // 10: dE = dH1 . DW1 ; dDW1 += dH1^T . X0      (the scatter group of the PREVIOUS tile must have drained the DE columns)
-      wait_epi();
-      if (it > 0 && !(a.dbg & 6)) {
-        const int64_t pt = it - 1;
-        mbar_wait(bar(B_DEEMPTY0 + (int)(pt & 1)), (uint32_t)((pt >> 1) & 1), a.status, 4, acc);
-        tc_fence_after();
-      }
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) umma(tmem + T_DE, dk_lo(h1, kk), dk_hi(64), dm_lo(w_dw1, 32, kk), dm_hi(), i_dg32, kk > 0, a.dbg & 64);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) umma(tmem + T_WDW1, dm_lo(h1, 64, kk), dm_hi(), dm_lo(x0, 32, kk), dm_hi(), i_wg32, kk > 0 ? 1u : acc_first, a.dbg & 64);
-        umma_commit(bar(B_DEFULL0 + s));
-        umma_commit(bar(B_EMPTY0 + s));  // the stage's encodings are not read any more
-      }
-      __syncwarp();
-    }
-    if (elect_one()) umma_commit(bar(B_WG));  // every weight-gradient GEMM of this CTA has completed
-    __syncwarp();
-  } else if (warp >= 4 && warp < 8) {
-    // ================================ epilogue ================================
-    const int row = (warp & 3) * 32 + lane;
-    const uint32_t lane_addr = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-    uint32_t p_mma = 0;
-    int tr_n = 2048;
-    int64_t tr_it = 0;
-    auto stamp = [&]() {
-      if (a.trace != nullptr && blockIdx.x == 0 && tid == 128 && tr_it >= 2 && tr_n < 4096) a.trace[tr_n++] = clock64();
-    };
-    auto wait_mma = [&]() {
-      mbar_wait(bar(B_MMA), p_mma, a.status, 5, acc);
-      p_mma ^= 1u;
-      tc_fence_after();
-      stamp();   // accumulator ready
-    };
-    auto signal = [&]() {  // my TMEM reads are done and my smem writes are visible to the tensor core
-      stamp();   // row computed and stored
-      tc_fence_before();
-      if (!(a.dbg & 16)) proxy_fence();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar(B_EPI));
-      stamp();   // handed back
-    };
-    for (int64_t it = 0; it < my_tiles; ++it) {
-      const int s = (int)(it & 1);
-      const int64_t tile = blockIdx.x + it * gridDim.x, grow = tile * kRows + row;
-      const bool live = grow < n;
+      const int64_t tile = blockIdx.x + it * gridDim.x;
       uint8_t* st = smem + STAGES + s * kStageBytes;
-      tr_it = it;
-      mbar_wait(bar(B_FULL0 + s), (uint32_t)((it >> 1) & 1), a.status, 6, acc);
-      const float* rf = reinterpret_cast<const float*>(st + S_XYZ) + row * 6;
-      const float dirx = rf[3], diry = rf[4], dirz = rf[5];
-      const float* rg = reinterpret_cast<const float*>(st + S_DRGB) + row * 3;
-      const float drgb0 = live ? rg[0] : 0.f, drgb1 = live ? rg[1] : 0.f, drgb2 = live ? rg[2] : 0.f;
-      const float dsraw = live ? reinterpret_cast<const float*>(st + S_DS)[row] : 0.f;
-      if (!live) {  // rows past the end hold whatever the buffers contained: keep 0 * NaN out of the weight-gradient sums
+      const uint32_t x0 = sbase + STAGES + (uint32_t)s * kStageBytes + S_X0 + c * 32 * 128;
+      const bool live[2] = {tile * kRows + rr[0] < n, tile * kRows + rr[1] < n};
+      const uint32_t keep[2] = {live[0] ? 0xFFFFFFFFu : 0u, live[1] ? 0xFFFFFFFFu : 0u};
+      mbar_wait(bar(B_FULL0 + s), (uint32_t)((it >> 1) & 1), a.status, 3);
+      float drgb[2][3], dsraw[2];
 #pragma unroll
-        for (int kc = 0; kc < 4; ++kc) *reinterpret_cast<uint4*>(st + S_X0 + canon_off(row, kc * 8, 32)) = make_uint4(0, 0, 0, 0);
+      for (int h = 0; h < 2; ++h) {
+        const float* rg = reinterpret_cast<const float*>(st + S_DRGB) + rr[h] * 3;
+#pragma unroll
+        for (int e = 0; e < 3; ++e) drgb[h][e] = live[h] ? rg[e] : 0.f;
+        dsraw[h] = live[h] ? reinterpret_cast<const float*>(st + S_DS)[rr[h]] : 0.f;
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar(B_EMPTY0 + s));
-      if (a.dbg & 8) continue;
-      {  // SH of the view direction -> columns 16..31 of the colour network's input
-        uint4 s0 = make_uint4(0, 0, 0, 0), s1 = s0;
-        if (live) {
+      {  // thread pair per row: SH of the view direction -> columns 16..31 of the colour network's input; rows past the end: zero
+         // encodings (the buffers hold whatever they contained: keep 0 * NaN out of the weight-gradient sums)
+        const int row = R0 + (t >> 1), part = t & 1;
+        const bool row_live = tile * kRows + row < n;
+        const float* rf = reinterpret_cast<const float*>(st + S_XYZ) + row * 6;
+        uint4 sv = make_uint4(0, 0, 0, 0);
+        if (row_live) {
           float sh[16];
-          nsr_sh4(dirx, diry, dirz, sh);
-          s0 = make_uint4(nsr_pack_h2(sh[0], sh[1]), nsr_pack_h2(sh[2], sh[3]), nsr_pack_h2(sh[4], sh[5]), nsr_pack_h2(sh[6], sh[7]));
-          s1 = make_uint4(nsr_pack_h2(sh[8], sh[9]), nsr_pack_h2(sh[10], sh[11]), nsr_pack_h2(sh[12], sh[13]), nsr_pack_h2(sh[14], sh[15]));
+          nsr_sh4(rf[3], rf[4], rf[5], sh);
+          const float* q = sh + 8 * part;
+          sv = make_uint4(nsr_pack_h2(q[0], q[1]), nsr_pack_h2(q[2], q[3]), nsr_pack_h2(q[4], q[5]), nsr_pack_h2(q[6], q[7]));
+        } else {
+          *reinterpret_cast<uint4*>(st + S_X0 + nsr_canon_off(row, 16 * part, 32)) = make_uint4(0, 0, 0, 0);
+          *reinterpret_cast<uint4*>(st + S_X0 + nsr_canon_off(row, 16 * part + 8, 32)) = make_uint4(0, 0, 0, 0);
         }
-        *reinterpret_cast<uint4*>(smem + A_CI + canon_off(row, 16, 32)) = s0;
-        *reinterpret_cast<uint4*>(smem + A_CI + canon_off(row, 24, 32)) = s1;
+        *reinterpret_cast<uint4*>(smem + A_CI + nsr_canon_off(row, 16 + 8 * part, 32)) = sv;
       }
-      // 1: H1 = relu(.)
-      wait_mma();
-      epi_hidden<0>(lane_addr, smem + A_H1, row, live, a.dbg & 32);
-      signal();
-      // 2: out16 (fp16) -> columns 0..15 of the colour input
-      wait_mma();
+      // 1: H1 = relu(X0 . DW1^T)
       {
-        uint32_t v[16];
-        tmem_ld16(lane_addr + T_ACC, v);
-        tmem_ld_wait();
-        uint32_t pk[8];
+        float d[32];
+        begin();
 #pragma unroll
-        for (int j = 0; j < 8; ++j) pk[j] = live ? nsr_pack_h2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1])) : 0u;
-        *reinterpret_cast<uint4*>(smem + A_CI + canon_off(row, 0, 32)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        *reinterpret_cast<uint4*>(smem + A_CI + canon_off(row, 8, 32)) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+        for (int kk = 0; kk < 2; ++kk) nsr_wgmma_n64<0, 0>(d, dk(x0, 32, kk), dk(w_dw1, 32, kk), kk > 0);
+        end();
+        nsr_wg_fence_regs(d);
+        epi64<0>(d, smem + A_H1, rr, keep, c0);
       }
-      signal();
-      // 3, 4: colour hidden layers
-      wait_mma();
-      epi_hidden<0>(lane_addr, smem + A_G1, row, live, a.dbg & 32);
-      signal();
-      wait_mma();
-      epi_hidden<0>(lane_addr, smem + A_G2, row, live, a.dbg & 32);
-      signal();
-      // 5: d(rgb pre-activation) = d_rgb * s (1 - s), s = sigmoid(fp16(raw)); columns 0..2, the rest of the 16-wide operand is zero
-      wait_mma();
+      // 2: out16 = H1 . DW2^T (fp16) -> columns 0..15 of the colour input
       {
-        uint32_t v[16];
-        tmem_ld16(lane_addr + T_ACC, v);
-        tmem_ld_wait();
-        float dp[3];
-        const float dr[3] = {drgb0, drgb1, drgb2};
+        float d[8];
+        begin();
 #pragma unroll
-        for (int e = 0; e < 3; ++e) {
-          const float raw = __half2float(__float2half_rn(__uint_as_float(v[e])));
-          const float sg = 1.f / (1.f + expf(-raw));
-          dp[e] = live ? dr[e] * sg * (1.f - sg) * loss_scale : 0.f;
-        }
-        *reinterpret_cast<uint4*>(smem + A_DC3 + canon_off(row, 0, 16)) = make_uint4(nsr_pack_h2(dp[0], dp[1]), nsr_pack_h2(dp[2], 0.f), 0u, 0u);
-        *reinterpret_cast<uint4*>(smem + A_DC3 + canon_off(row, 8, 16)) = make_uint4(0u, 0u, 0u, 0u);
+        for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n16<0, 0>(d, dk(h1, 64, kk), dk(w_dw2, 64, kk), kk > 0);
+        end();
+        nsr_wg_fence_regs(d);
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            *reinterpret_cast<uint32_t*>(smem + A_CI + nsr_canon_off(rr[h], 8 * j + c0, 32)) = nsr_pack_h2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]) & keep[h];
       }
-      signal();
-      // 6, 7: dgrad through the colour hidden layers (in place over G2, G1)
-      wait_mma();
-      epi_hidden<1>(lane_addr, smem + A_G2, row, live, a.dbg & 32);
-      signal();
-      wait_mma();
-      epi_hidden<1>(lane_addr, smem + A_G1, row, live, a.dbg & 32);
-      signal();
-      // 8: d(out16) = colour path + d sigma_raw on column 0
-      wait_mma();
+      // 3, 4: colour hidden layers G1 = relu([O | SH] . CW1^T), G2 = relu(G1 . CW2^T)
       {
-        uint32_t v[16];
-        tmem_ld16(lane_addr + T_ACC, v);
-        tmem_ld_wait();
-        float f0 = __uint_as_float(v[0]) + dsraw * loss_scale;
-        uint32_t pk[8];
-        pk[0] = nsr_pack_h2(f0, __uint_as_float(v[1]));
+        float d[32];
+        begin();
 #pragma unroll
-        for (int j = 1; j < 8; ++j) pk[j] = nsr_pack_h2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-        if (!live) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) pk[j] = 0u;
-        }
-        *reinterpret_cast<uint4*>(smem + A_DO + canon_off(row, 0, 16)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        *reinterpret_cast<uint4*>(smem + A_DO + canon_off(row, 8, 16)) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+        for (int kk = 0; kk < 2; ++kk) nsr_wgmma_n64<0, 0>(d, dk(ci, 32, kk), dk(w_cw1, 32, kk), kk > 0);
+        end();
+        nsr_wg_fence_regs(d);
+        epi64<0>(d, smem + A_G1, rr, keep, c0);
       }
-      signal();
-      // 9: dgrad through the density hidden layer (in place over H1)
-      wait_mma();
-      epi_hidden<1>(lane_addr, smem + A_H1, row, live, a.dbg & 32);
-      signal();
-    }
-    // ---- weight gradients: TMEM -> global (M = 64 accumulators live in lanes 0..15 of every 32-lane quarter: row = 16 * quarter + lane)
-    if (my_tiles > 0 && !(a.dbg & 8)) {
-      mbar_wait(bar(B_WG), 0u, a.status, 7, acc);
-      tc_fence_after();
-      const int q = warp & 3, m = 16 * q + lane;
-      auto flush = [&](uint32_t col0, int ncols, float* dst, int stride_m, int stride_c) {
-        for (int c0 = 0; c0 < ncols; c0 += 16) {
-          uint32_t v[16];
-          tmem_ld16(lane_addr + col0 + (uint32_t)c0, v);
-          tmem_ld_wait();
-          if (lane < 16) {
+      {
+        float d[32];
+        begin();
 #pragma unroll
-            for (int j = 0; j < 16; ++j) atomicAdd(dst + (size_t)m * stride_m + (size_t)(c0 + j) * stride_c, __uint_as_float(v[j]) * inv_scale);
+        for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n64<0, 0>(d, dk(g1, 64, kk), dk(w_cw2, 64, kk), kk > 0);
+        end();
+        nsr_wg_fence_regs(d);
+        epi64<0>(d, smem + A_G2, rr, keep, c0);
+      }
+      // 5: rgb_pre = G2 . CW3^T; d(rgb pre-activation) = d_rgb * s (1 - s), s = sigmoid(fp16(raw)) on columns 0..2, zero elsewhere
+      {
+        float d[8];
+        begin();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n16<0, 0>(d, dk(g2, 64, kk), dk(w_cw3, 64, kk), kk > 0);
+        end();
+        nsr_wg_fence_regs(d);
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float dp[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = 8 * j + c0 + e;
+              dp[e] = 0.f;
+              if (col < 3) {
+                const float raw = __half2float(__float2half_rn(d[4 * j + 2 * h + e]));
+                const float sg = 1.f / (1.f + expf(-raw));
+                const float dr = col == 0 ? drgb[h][0] : (col == 1 ? drgb[h][1] : drgb[h][2]);
+                dp[e] = live[h] ? dr * sg * (1.f - sg) * loss_scale : 0.f;
+              }
+            }
+            *reinterpret_cast<uint32_t*>(smem + A_DC3 + nsr_canon_off(rr[h], 8 * j + c0, 16)) = nsr_pack_h2(dp[0], dp[1]);
           }
+      }
+      // 6: dG2pre = dC3 . CW3 ; dCW3^T += G2^T . dC3 ; dG2 in place over G2
+      {
+        {
+          float w[8];
+          begin();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n16<1, 1>(w, dm(g2, 64, kk), dm(dc3, 16, kk), kk > 0);
+          end();
+          nsr_wg_fence_regs(w);
+          wacc_add(wacc, G_CW3, t, w);
+        }
+        float d[32];
+        nsr_wg_fence();
+        nsr_wgmma_n64<0, 1>(d, dk(dc3, 16, 0), dm(w_cw3, 64, 0), 0u);
+        end();
+        nsr_wg_fence_regs(d);
+        epi64<1>(d, smem + A_G2, rr, keep, c0);
+      }
+      // 7: dG1pre = dG2 . CW2 ; dCW2 += dG2^T . G1 ; dG1 in place over G1
+      {
+        {
+          float w[32];
+          begin();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n64<1, 1>(w, dm(g2, 64, kk), dm(g1, 64, kk), kk > 0);
+          end();
+          nsr_wg_fence_regs(w);
+          wacc_add(wacc, G_CW2, t, w);
+        }
+        float d[32];
+        nsr_wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n64<0, 1>(d, dk(g2, 64, kk), dm(w_cw2, 64, kk), kk > 0);
+        end();
+        nsr_wg_fence_regs(d);
+        epi64<1>(d, smem + A_G1, rr, keep, c0);
+      }
+      // 8: dOpre = dG1 . CW1[:, 0:16] ; dCW1 += dG1^T . CI ; d(out16) = colour path + d sigma_raw on column 0
+      {
+        {
+          float w[16];
+          begin();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n32<1, 1>(w, dm(g1, 64, kk), dm(ci, 32, kk), kk > 0);
+          end();
+          nsr_wg_fence_regs(w);
+          wacc_add(wacc, G_CW1, t, w);
+        }
+        float d[8];
+        nsr_wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n16<0, 1>(d, dk(g1, 64, kk), dm(w_cw1, 32, kk), kk > 0);
+        end();
+        nsr_wg_fence_regs(d);
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float f0 = d[4 * j + 2 * h] + (j == 0 && c0 == 0 ? dsraw[h] * loss_scale : 0.f);
+            *reinterpret_cast<uint32_t*>(smem + A_DO + nsr_canon_off(rr[h], 8 * j + c0, 16)) = nsr_pack_h2(f0, d[4 * j + 2 * h + 1]) & keep[h];
+          }
+      }
+      // 9: dH1pre = dO . DW2 ; dDW2^T += H1^T . dO ; dH1 in place over H1
+      {
+        {
+          float w[8];
+          begin();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n16<1, 1>(w, dm(h1, 64, kk), dm(dO, 16, kk), kk > 0);
+          end();
+          nsr_wg_fence_regs(w);
+          wacc_add(wacc, G_DW2, t, w);
+        }
+        float d[32];
+        nsr_wg_fence();
+        nsr_wgmma_n64<0, 1>(d, dk(dO, 16, 0), dm(w_dw2, 64, 0), 0u);
+        end();
+        nsr_wg_fence_regs(d);
+        epi64<1>(d, smem + A_H1, rr, keep, c0);
+      }
+      // 10: dE = dH1 . DW1 ; dDW1 += dH1^T . X0 -> d(encoding) slot s (the scatter group of tile it - 2 must have drained it)
+      {
+        {
+          float w[16];
+          begin();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n32<1, 1>(w, dm(h1, 64, kk), dm(x0, 32, kk), kk > 0);
+          end();
+          nsr_wg_fence_regs(w);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bar(B_EMPTY0 + s));  // the stage's inputs are not read any more
+          wacc_add(wacc, G_DW1, t, w);
+        }
+        float d[16];
+        nsr_wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) nsr_wgmma_n32<0, 1>(d, dk(h1, 64, kk), dm(w_dw1, 32, kk), kk > 0);
+        end();
+        nsr_wg_fence_regs(d);
+        if (it >= 2) mbar_wait(bar(B_DEEMPTY0 + s), (uint32_t)(((it - 2) >> 1) & 1), a.status, 4);
+        uint32_t* de = reinterpret_cast<uint32_t*>(smem + DE + s * kDeBytes);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) de[rr[h] * DE_STRIDE + 4 * j + (lane & 3)] = nsr_pack_h2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar(B_DEFULL0 + s));
+      }
+    }
+    // ---- weight gradients: shared accumulator -> global, slots split between the two warpgroups
+    chain_bar();
+    if (my_tiles > 0) {
+      auto flush = [&](int slot0, int N, float* dst, int stride_m, int stride_n) {
+        for (int r = c; r < N / 2; r += 2) {
+          const int j = r >> 2, h = (r >> 1) & 1, e = r & 1;
+          const int m = 16 * (warp & 3) + (lane >> 2) + 8 * h, col = 8 * j + c0 + e;
+          atomicAdd(dst + (size_t)m * stride_m + (size_t)col * stride_n, wacc[(slot0 + r) * 128 + t] * inv_scale);
         }
       };
-      flush(T_WDW1, 32, a.grad_dparams, 32, 1);                     // dDW1 [out m][in c]
-      flush(T_WDW2, 16, a.grad_dparams + 64 * 32, 1, 64);           // dDW2^T [in m][out c] -> DW2 [out][in]
-      flush(T_WCW1, 32, a.grad_cparams, 32, 1);                     // dCW1 [out m][in c]
-      flush(T_WCW2, 64, a.grad_cparams + 64 * 32, 64, 1);           // dCW2 [out m][in c]
-      flush(T_WCW3, 16, a.grad_cparams + 64 * 32 + 64 * 64, 1, 64); // dCW3^T [in m][out c] -> CW3 [out][in]
-      tc_fence_before();
+      flush(G_DW1, 32, a.grad_dparams, 32, 1);                     // dDW1 [out m][in n]
+      flush(G_DW2, 16, a.grad_dparams + 64 * 32, 1, 64);           // dDW2^T [in m][out n] -> DW2 [out][in]
+      flush(G_CW1, 32, a.grad_cparams, 32, 1);                     // dCW1 [out m][in n]
+      flush(G_CW2, 64, a.grad_cparams + 64 * 32, 64, 1);           // dCW2 [out m][in n]
+      flush(G_CW3, 16, a.grad_cparams + 64 * 32 + 64 * 64, 1, 64); // dCW3^T [in m][out n] -> CW3 [out][in]
     }
-  } else if (warp >= 8) {
+  } else {
     // ================================ scatter ================================
     const int grp = (warp - 8) >> 2;  // tiles alternate between the two groups
     const int row = (warp & 3) * 32 + lane;
-    const uint32_t lane_addr = tmem + ((uint32_t)((warp & 3) * 32) << 16);
+    const bool loader = (warp & 3) == 0 && lane == 0;
     float* grad_table = a.grad_dparams + NF_DENSITY_PARAMS;
+    auto load = [&](int64_t it) {  // tile inputs of the CTA's tile `it` -> stage it & 1
+      const int64_t tile = blockIdx.x + it * gridDim.x, row0 = tile * kRows;
+      const uint32_t dst = sbase + STAGES + (uint32_t)(it & 1) * kStageBytes, fb = bar(B_FULL0 + (int)(it & 1));
+      mbar_expect_tx(fb, kStageBytes);
+      tma_bulk(dst + S_X0, a.enc_tiles + tile * (kRows * 32 * 2), kRows * 32 * 2, fb);
+      tma_bulk(dst + S_XYZ, a.xyzdir + row0 * 6, kRows * 6 * 4, fb);
+      tma_bulk(dst + S_DS, a.d_sraw + row0, kRows * 4, fb);
+      tma_bulk(dst + S_DRGB, a.d_rgb + row0 * 3, kRows * 3 * 4, fb);
+    };
+    if (loader && grp < my_tiles) load(grp);
     for (int64_t it = grp; it < my_tiles; it += 2) {
       const int s = (int)(it & 1);  // == grp
       const int64_t tile = blockIdx.x + it * gridDim.x, grow = tile * kRows + row;
       const bool ok = grow < n;
       const uint8_t* st = smem + STAGES + s * kStageBytes;
-      mbar_wait(bar(B_FULL0 + s), (uint32_t)((it >> 1) & 1), a.status, 8, acc);
+      mbar_wait(bar(B_FULL0 + s), (uint32_t)((it >> 1) & 1), a.status, 8);
       const float* rf = reinterpret_cast<const float*>(st + S_XYZ) + row * 6;
       const float x = rf[0], y = rf[1], z = rf[2];
       __syncwarp();
       if (lane == 0) mbar_arrive(bar(B_EMPTY0 + s));
-      if (a.dbg & 4) continue;
-      if (!(a.dbg & 2)) mbar_wait(bar(B_DEFULL0 + s), (uint32_t)((it >> 1) & 1), a.status, 9, acc);
-      tc_fence_after();
+      mbar_wait(bar(B_DEFULL0 + s), (uint32_t)((it >> 1) & 1), a.status, 9);
       uint32_t de[16];  // (feature 0, feature 1) of level l as fp16 pair, still multiplied by the loss scale
       {
-        uint32_t v[16];
-        tmem_ld16(lane_addr + T_DE, v);
-        tmem_ld_wait();
+        const uint4* src = reinterpret_cast<const uint4*>(smem + DE + s * kDeBytes + row * DE_STRIDE * 4);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) de[j] = nsr_pack_h2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
-        tmem_ld16(lane_addr + T_DE + 16u, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) de[8 + j] = nsr_pack_h2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
+        for (int q = 0; q < 4; ++q) {
+          const uint4 v = src[q];
+          de[4 * q] = v.x;
+          de[4 * q + 1] = v.y;
+          de[4 * q + 2] = v.z;
+          de[4 * q + 3] = v.w;
+        }
       }
-      if (a.dbg & 128) {  // timing experiments without the chain: a non-zero synthetic gradient so that every RED is issued
-#pragma unroll
-        for (int j = 0; j < 16; ++j) de[j] = 0x2C003400u + (uint32_t)((row + j) & 7);
-      }
-      tc_fence_before();
       __syncwarp();
       if (lane == 0) mbar_arrive(bar(B_DEEMPTY0 + s));
+      if (loader && it + 2 < my_tiles) {  // every reader of this tile's stage has arrived: refill it with the group's next tile
+        mbar_wait(bar(B_EMPTY0 + s), (uint32_t)((it >> 1) & 1), a.status, 1);
+        load(it + 2);
+      }
 #pragma unroll
       for (int l = 0; l < 16; ++l) {
         float2 d = __half22float2(*reinterpret_cast<const __half2*>(&de[l]));
@@ -643,10 +504,10 @@ __global__ void __launch_bounds__(kThreads, 2) nerf_bwd_tc_kernel(const __grid_c
         nsr_pos_fract(z, li.scale, cz, fz);
         float v[16];
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const float w = nsr_corner_weight(c, fx, fy, fz);
-          v[2 * c] = w * d.x;
-          v[2 * c + 1] = w * d.y;
+        for (int cc = 0; cc < 8; ++cc) {
+          const float w = nsr_corner_weight(cc, fx, fy, fz);
+          v[2 * cc] = w * d.x;
+          v[2 * cc + 1] = w * d.y;
         }
         bool issue = ok && (d.x != 0.f || d.y != 0.f);
         if (l < 8) {  // runs of consecutive samples in one cell: sum across the warp, the last lane of a run issues
@@ -672,22 +533,19 @@ __global__ void __launch_bounds__(kThreads, 2) nerf_bwd_tc_kernel(const __grid_c
           }
           issue = ok && tail;
         }
-        if (issue && !(a.dbg & 1)) {
+        if (issue) {
           nsr_corner_indices(li, cx, cy, cz, idx);
 #pragma unroll
-          for (int c = 0; c < 8; c += 2) nsr_red_corner_pair(grad_table, idx[c], idx[c + 1], v[2 * c], v[2 * c + 1], v[2 * c + 2], v[2 * c + 3]);
+          for (int cc = 0; cc < 8; cc += 2) nsr_red_corner_pair(grad_table, idx[cc], idx[cc + 1], v[2 * cc], v[2 * cc + 1], v[2 * cc + 2], v[2 * cc + 3]);
         }
       }
     }
   }
-  if (acc != nullptr) acc[0] = clock64() - t_begin;
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 256;" ::"r"(tmem) : "memory");
 }
 
 }  // namespace
 
-// tcgen05 / TMA form of nsr_nerf_field_bwd over the packed inputs.  enc_tiles_h: the kept samples' encodings in the canonical tile layout
+// wgmma / TMA form of nsr_nerf_field_bwd over the packed inputs.  enc_tiles_h: the kept samples' encodings in the canonical tile layout
 // (nsr_pack_kept with enc_tiled = 1: tile t = rows [128 t, 128 t + 128), 8 KB each); xyzdir / d_sraw / d_rgb in packed row order.  All four
 // buffers must be readable up to the end of the last 128-row tile (the kernel masks rows >= k itself).  status (device int, may be NULL)
 // receives a non-zero code if an mbarrier wait timed out (the kernel then traps instead of hanging).
@@ -723,28 +581,10 @@ extern "C" int nsr_nerf_field_bwd_tc(const nsr_nerf_t* f, const void* enc_tiles_
   a.n_cap = k;
   a.loss_scale = loss_scale;
   a.status = status;
-  static const int dbg = [] { const char* v = getenv("NSR_TC_DEBUG"); return v ? atoi(v) : 0; }();
-  a.dbg = dbg;
-  static const char* trace_path = getenv("NSR_TC_TRACE");   // development aid: dump CTA 0's pipeline time stamps after a synchronised launch
-  static long long* trace_dev = nullptr;
-  if (trace_path != nullptr && trace_dev == nullptr) {
-    cudaMalloc(&trace_dev, 4096 * sizeof(long long));
-  }
-  if (trace_dev != nullptr) cudaMemsetAsync(trace_dev, 0, 4096 * sizeof(long long), (cudaStream_t)stream);
-  a.trace = trace_dev;
   const int64_t tiles = (k + kRows - 1) / kRows;
-  int grid = (int)min((int64_t)nsr_sm_count() * 2, tiles);
-  if (k_dev != nullptr) grid = nsr_sm_count() * 2;
+  int grid = (int)min((int64_t)nsr_sm_count(), tiles);
+  if (k_dev != nullptr) grid = nsr_sm_count();
   nerf_bwd_tc_kernel<<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(*f, a);
   NSR_CHECK_LAUNCH("nsr_nerf_field_bwd_tc");
-  if (trace_dev != nullptr) {
-    static long long host[4096];
-    cudaStreamSynchronize((cudaStream_t)stream);
-    cudaMemcpy(host, trace_dev, sizeof(host), cudaMemcpyDeviceToHost);
-    if (FILE* f = fopen(trace_path, "w")) {
-      for (int i = 0; i < 4096; ++i) fprintf(f, "%lld\n", host[i]);
-      fclose(f);
-    }
-  }
   return 0;
 }

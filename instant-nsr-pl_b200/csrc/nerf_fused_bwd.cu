@@ -388,8 +388,8 @@ namespace {
 // Per level: corner weights x d(feature pair); on levels < kMergeLevels runs of rows that sit in the same cell (consecutive samples of
 // a ray on the coarse levels) are summed with a segmented shuffle scan over the whole warp and only the run's last lane issues REDs;
 // x-adjacent corners that are neighbours in memory (hashed levels: cell x even; dense levels: entry index even) leave as ONE 16-byte
-// red.global.add.v4.f32.  48 registers, no shared memory: 64 warps per SM keep the RED path of the SM full (tools/gather_bench.py,
-// profiles/r2_scatter_microbench.md: 92 us for 267 k samples against 264 us for the plain 8-byte form).
+// red.global.add.v4.f32.  48 registers, no shared memory: 64 warps per SM keep the RED path of the SM full (tools/gather_bench.py times
+// this form against the plain 8-byte REDs).
 constexpr int kMergeLevels = 8;
 
 template <int MINB>   // resident CTAs per SM the register allocation is sized for: 5 (48 registers), 6 (40), 8 (32, 64 B of spills)

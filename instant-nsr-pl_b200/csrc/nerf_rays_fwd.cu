@@ -65,7 +65,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 }
 
 // MINB = resident CTAs per SM the register allocation is sized for: 2 (128 registers).  (A 3-CTA instantiation -- 80 registers, 0.5 KB of
-// spills per thread, 24 warps per SM -- was timed in round 2: 196 us against 131 us, and removed.)
+// spills per thread, 24 warps per SM -- was markedly slower and is not built.)
 template <int MINB, int NB>
 __global__ void __launch_bounds__(kThreads, MINB) nerf_rays_fwd_kernel(const __grid_constant__ nsr_nerf_t P, const RaysFwdArgs a) {
   extern __shared__ __align__(16) __half smem[];
@@ -344,7 +344,7 @@ __global__ void __launch_bounds__(256) pack_kept_kernel(const int64_t* __restric
   if (enc_k && !enc_tiled) {  // 64 B rows: 4 lanes per row => every warp iteration moves 8 whole rows with fully used sectors
     for (int64_t v = lane; v < cnt * 4; v += 32) enc_k[dst * 4 + v] = enc_loose[src * 4 + v];
   } else if (enc_k) {
-    // canonical UMMA tile layout for the tcgen05 backward (csrc/nerf_bwd_tc.cu): packed row R lives in tile R / 128 (8 KB each); inside a
+    // canonical tensor-core tile layout for the wgmma backward (csrc/nerf_bwd_tc.cu): packed row R lives in tile R / 128 (8 KB each); inside a
     // tile the 16-byte chunk (row r, k chunk kc) sits at ((r / 8) * 4 + kc) * 128 + (r % 8) * 16 bytes -- ONE cp.async.bulk then fetches a tile
     for (int64_t v = lane; v < cnt * 4; v += 32) {
       const int64_t R = dst + (v >> 2);

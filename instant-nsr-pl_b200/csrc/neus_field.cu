@@ -163,8 +163,7 @@ __global__ void __launch_bounds__(kThreads, 3) neus_field_fwd_kernel(const __gri
 }
 
 // ---- forward with the three GEMMs of the SDF network on tensor cores ---------------------------------------------------------
-// ncu (round 2, profiles/r2_ncu_final.md): the thread-per-sample kernel above executes 15.6 k warp instructions per 32 samples, more than
-// half of them the 64 x (36 + 16 + 36) scalar FMAs of  z = W1 e,  out = W2 h,  q = W1^T u  with their weight loads from shared memory.
+// The thread-per-sample kernel above spends more than half of its instructions on the 64 x (36 + 16 + 36) scalar FMAs of  z = W1 e,  out = W2 h,  q = W1^T u  with their weight loads from shared memory.
 // Here a warp owns 32 samples; the gathers stay thread-per-sample, the three products run as m16n8k16 MMAs with fp32 accumulation on
 // operands SPLIT into fp16 hi + lo parts (x = hi + lo, hi = fp16(x), lo = fp16(x - hi)):  x w ~= hi_x hi_w + lo_x hi_w + hi_x lo_w, i.e.
 // ~21 bits of every product survive (the dropped lo_x lo_w term is 2^-22 relative): fp32-level accuracy for the inv_s-amplified SDF,
@@ -495,8 +494,8 @@ __global__ void __launch_bounds__(kThreads, 2) neus_field_bwd_kernel(const __gri
     for (int o = 0; o < NOUTP; ++o) T[TT_GO + o * LDT + tid] = __float2half(go[o] * scale);
     // ---- table gradient: first- and second-order terms in one RED per corner.
     // Levels 0..kMergeLevels-1 can merge runs of equal cells across neighbouring lanes (consecutive samples of a ray) with a segmented
-    // warp scan so that only the last lane of a run issues the 8 REDs (as in nerf_fused_bwd.cu).  Measured on B200 (C3, 313 k samples):
-    // 8 merged levels 0.617 ms vs 0.558 ms without -- with one sample per thread the 85 shuffles per level cost more than the REDs
+    // warp scan so that only the last lane of a run issues the 8 REDs (as in nerf_fused_bwd.cu).  Merging was measured
+    // slower than plain REDs here -- with one sample per thread the 85 shuffles per level cost more than the REDs
     // they save (this kernel is not RED-bound), so merging is compiled out.
     constexpr int kMergeLevels = 0;
 #pragma unroll
@@ -642,10 +641,10 @@ extern "C" int nsr_neus_field_fwd(const nsr_grid_t* g, const float* points, cons
   if (int e = check(g, n_out, "nsr_neus_field_fwd")) return e;
   if (n == 0) return 0;
   // Default: neus_field_fwd_tc_kernel (SDF network on tensor cores, hi / lo split operands; same results to ~1e-6, every NeuS parity test
-  // runs on it).  Measured on B200 (C3, 313 k samples): 0.233 ms against 0.302 ms for the thread-per-sample kernel (NSR_NEUS_FWD=scalar).
-  // Its first version (three CTAs per SM, separate q tile) was SLOWER, 0.325 ms: the kernel is bound by the latency of its two gathers,
-  // and fewer instructions only paid once the freed registers / shared memory bought a fourth CTA per SM (q aliased onto the encoding rows).
-  // (Issuing the corner loads of four levels together in both gathers, as the NeRF forward does, was measured too: 0.247 ms, not kept.)
+  // runs on it); NSR_NEUS_FWD=scalar selects the thread-per-sample kernel.
+  // The kernel is bound by the latency of its two gathers: fewer instructions only pay once the freed registers / shared memory buy a
+  // fourth CTA per SM (q aliased onto the encoding rows).  Issuing the corner loads of four levels together, as the NeRF forward does,
+  // was not faster and is not kept.
   static const bool scalar = [] {
     const char* v = getenv("NSR_NEUS_FWD");
     return v != nullptr && v[0] == 's';

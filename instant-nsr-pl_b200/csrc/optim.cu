@@ -130,7 +130,7 @@ extern "C" int nsr_adamw_step(const nsr_adamw_t* h, float* params, const float* 
   c.inv_scale = h->inv_grad_scale;
   c.lr = h->lr;
   c.weight_decay = h->weight_decay;
-  // launch shape: NSR_ADAMW_VARIANT = "<unroll 1|2|4>,<ctas per SM, 0 = one CTA per chunk>" (development knob; default = the fastest of tools/adamw_bench.py's sweep on B200: 5.86 TB/s)
+  // launch shape: NSR_ADAMW_VARIANT = "<unroll 1|2|4>,<ctas per SM, 0 = one CTA per chunk>" (development knob; tools/adamw_bench.py sweeps it)
   static int unroll = 1, ctas_per_sm = 0;
   static bool read_env = false;
   if (!read_env) {

@@ -107,8 +107,8 @@ __global__ void __launch_bounds__(256) p2p_allreduce_mean_multimem_kernel(float*
 }
 
 // ---- one-launch exchange: entry barrier + reduce-scatter + all-gather + exit barrier in ONE kernel ------------------------------------
-// (round 1 used three launches -- barrier, reduce, barrier -- plus a 50 MB copy into the symmetric buffer; the step's backward now
-//  accumulates straight into that buffer and this kernel is the whole exchange.)
+// (The step's backward accumulates straight into the symmetric buffer, so this kernel is the whole exchange: no separate barrier
+//  launches and no 50 MB copy-in.)
 //   entry : CTA 0 publishes "rank's gradients are complete" (epoch e) into every peer's flag array; EVERY CTA waits until all peers have
 //           published e (their backward kernels are behind them) -- no grid-wide sync needed, each CTA polls the local flags itself
 //   data  : rank r owns chunk r; U 16-byte columns per thread are in flight before the first is consumed

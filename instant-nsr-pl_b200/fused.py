@@ -139,7 +139,7 @@ class _NerfRenderRays(torch.autograd.Function):
         # plus (training, tile backward) the backward's inputs in packed row order: encodings, unit-cube position + view direction
         ri, ts, te, pos = i32(cap), f32(cap), f32(cap), i64(cap)
         packed_bwd = need_grad and fused.bwd_kernel in ('tiles', 'tiles_split', 'tc') and fused.packed_bwd_inputs
-        tiled = 1 if fused.bwd_kernel == 'tc' else 0   # tcgen05 backward: encodings in canonical 128-row UMMA tiles (one TMA bulk copy per tile)
+        tiled = 1 if fused.bwd_kernel == 'tc' else 0   # tensor-core backward: encodings in canonical 128-row tiles (one TMA bulk copy per tile)
         # (+pad rows: the tile backwards prefetch whole tiles -- 64 rows with cp.async, 128 rows with cp.async.bulk -- the last one may reach past K)
         pad = 256 - cap % 128 if tiled else 64
         enc_k = torch.empty(cap + pad, 32, dtype=torch.float16, device=dev) if packed_bwd else None
@@ -195,7 +195,7 @@ class _NerfRenderRays(torch.autograd.Function):
                          ptr(rgbs), ptr(f32(g_rgb)), ptr(f32(g_op)), ptr(f32(g_depth)), ptr(f32(g_w)), ptr(d_sraw), ptr(d_rgb), ptr(amax),
                          ptr(offsets_k) if packed else None, n, stream())
                 if packed and fused.bwd_kernel == 'tc':
-                    # Blackwell-native backward: tcgen05 GEMM chain + TMA-staged tiles + scatter warps in one kernel (csrc/nerf_bwd_tc.cu)
+                    # Hopper tensor-core backward: wgmma GEMM chain + TMA-staged tiles + scatter warps in one kernel (csrc/nerf_bwd_tc.cu)
                     if fused._tc_status is None or fused._tc_status.device != dev:
                         fused._tc_status = torch.zeros(1, dtype=torch.int32, device=dev)
                     lib.call('nsr_nerf_field_bwd_tc', fused.ref(), ptr(enc_k), ptr(dh), ptr(ch), ptr(d_sraw), ptr(d_rgb), ptr(gd), ptr(gc),
@@ -252,8 +252,8 @@ class NerfFused:
         self.packed_bwd_inputs = True   # tile backward reads its inputs in packed row order (written by nsr_pack_kept)
         from .config import experimental
         self.fuse_kept_scan = experimental('pack_scan')   # nsr_pack_kept_scan instead of nsr_scan_counts + nsr_pack_kept (not yet timed)
-        # 'tiles_split' (default: network half + high-occupancy table scatter, 189 us) | 'tiles' (one sample-tile backward kernel, REDs from the
-        # MMA warps, 202 us) | 'tc' (tcgen05 / TMA warp-specialised kernel, 208 us: csrc/nerf_bwd_tc.cu) | 'rays' (single per-ray backward kernel)
+        # 'tiles_split' (default: network half + high-occupancy table scatter) | 'tiles' (one sample-tile backward kernel, REDs from the
+        # MMA warps) | 'tc' (wgmma / TMA warp-specialised kernel: csrc/nerf_bwd_tc.cu) | 'rays' (single per-ray backward kernel)
         import os
         self.bwd_kernel = os.environ.get('NSR_BWD_KERNEL', 'tiles_split')
         self._tc_status = None
@@ -262,8 +262,8 @@ class NerfFused:
         # the marcher allocates every ray's rows and queue slot itself (nsr_march_rays_alloc) instead of a one-CTA scan kernel behind it
         self.march_alloc = os.environ.get('NSR_MARCH_ALLOC', '1') == '1'
         self.direct_grads = None
-        # zero the backward's gradient buffers beside the forward on a side stream instead of in front of the backward.  Measured on B200:
-        # 0.411 vs 0.401 ms/step -- the fill kernel takes SMs from the persistent forward kernel at its launch -- so it stays opt-in.
+        # zero the backward's gradient buffers beside the forward on a side stream instead of in front of the backward: opt-in, because
+        # the fill kernel takes SMs from the persistent forward kernel at its launch.
         self.prezero_grads = os.environ.get('NSR_PREZERO_GRADS', '0') == '1'
         self._side = None
         self._want_grad = True

@@ -1,4 +1,4 @@
-"""CUDA-graph execution of a whole training step (B200-first replacement for launching ~40 small kernels per
+"""CUDA-graph execution of a whole training step (replacement for launching ~40 small kernels per
 step from Python: the reference's per-step host cost dominates once the kernels take well under a millisecond).
 
     step = GraphedStep(model, loss_fn, n_rays, batch_spec={'rgb': (3,)})

@@ -102,7 +102,7 @@ class MlpSpec:
         if otype not in ('FullyFusedMLP', 'CutlassMLP'):
             raise NotImplementedError(f'network otype={otype!r} not implemented')
         self.n_in, self.n_out = int(n_in), int(n_out)
-        # 'mma_sync' (warp-level tensor cores, default) | 'tcgen05' (5th-gen tensor cores + TMEM; forward only, our extension key)
+        # 'mma_sync' (warp-level tensor cores, default) | 'wgmma' (Hopper warpgroup MMA from shared memory; forward only, our extension key)
         self.backend = str(cfg.get('backend', os.environ.get('NSR_MLP_BACKEND', 'mma_sync')))
         self.n_neurons = int(cfg.get('n_neurons', 64))
         self.n_hidden = int(cfg.get('n_hidden_layers', 1))
@@ -228,7 +228,7 @@ class _MlpFn(torch.autograd.Function):
     def forward(ctx, spec, x_h, params_f32, params_h):
         n = x_h.shape[0]
         out = torch.empty(n, 16, dtype=torch.float16, device=x_h.device)
-        if getattr(spec, 'backend', 'mma_sync') == 'tcgen05':   # tcgen05.mma + TMEM forward (bit-identical results)
+        if getattr(spec, 'backend', 'mma_sync') == 'wgmma':   # wgmma.mma_async forward (bit-identical results)
             lib.call('nsr_mlp_fwd_tc', spec.ref(), ptr(x_h), ptr(params_h), ptr(out), n, 0, None, stream())
         else:
             lib.call('nsr_mlp_fwd', spec.ref(), ptr(x_h), ptr(params_h), ptr(out), n, stream())

@@ -109,8 +109,8 @@ class P2PGradSync:
         self._peer = A(*[int(x) for x in self.hdl.buffer_ptrs])
         self._fpeer = A(*[int(x) for x in self.fhdl.buffer_ptrs])
         mc = int(getattr(self.hdl, 'multicast_ptr', 0) or 0)
-        # NVSwitch multicast reduce (multimem.ld_reduce / multimem.st): NSR_P2P_MULTIMEM = 1 | 0 | auto.  Measured on 2 x B200: plain P2P
-        # loads/stores 0.118 ms vs 0.17 ms through the multicast mapping for the 50 MB exchange, so auto uses it only from 4 ranks up
+        # NVSwitch multicast reduce (multimem.ld_reduce / multimem.st): NSR_P2P_MULTIMEM = 1 | 0 | auto.  At 2 ranks plain P2P
+        # loads/stores beat the multicast mapping for the 50 MB exchange, so auto uses it only from 4 ranks up
         # (in-switch reduction moves 1/world of the bytes per GPU).
         import os
         # NSR_P2P_EXCHANGE = fused (default: barriers inside the one reduce kernel, nsr_p2p_exchange_mean) | legacy (barrier, reduce, barrier)

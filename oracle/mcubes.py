@@ -1,7 +1,7 @@
 """Marching cubes -- CPU oracle (pure Python over the surface cells + numpy; small grids only).
 
 What it restates: ``MarchingCubeHelper.forward`` + ``isosurface_`` of models/geometry.py:32-104, whose arithmetic is the third-party
-``mcubes.marching_cubes`` (PyMCubes, requirements.txt:11 ``PyMCubes``, unpinned, NOT under /root/reference and not installed here).
+``mcubes.marching_cubes`` (PyMCubes, requirements.txt:11 ``PyMCubes``, unpinned, NOT under the reference repository and not installed here).
 PARITY UNPINNED against PyMCubes itself: a marching-cubes mesh is defined up to the triangulation of each cell, PyMCubes' vertex / face
 order is an implementation detail, and the reference ships no mesh fixtures.  What IS pinned, by tests/test_oracle_kat.py:
 closedness (every directed edge is balanced by an opposite one), outward orientation, vertices exactly on the trilinear

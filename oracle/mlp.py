@@ -23,7 +23,7 @@ class _RoundHalf(torch.autograd.Function):
     gradient to fp16 on the way back (the gradient of a half tensor is a half tensor) -- with an implicit loss scale of 1, so every
     gradient below the fp16 subnormal range (~3e-8) becomes exactly zero.  The reference never does that: tiny-cuda-nn multiplies its
     backward by loss_scale = 128 and Lightning's GradScaler by another 2^16 (SURVEY A.4 / A.6), i.e. its fp16 gradients do not
-    underflow at these magnitudes.  Found in round 2 by the 8192-ray parity test (per-sample gradients there are ~1e-8: 98 % of the
+    underflow at these magnitudes.  Found by the 8192-ray parity test (per-sample gradients there are ~1e-8: 98 % of the
     oracle's level-15 table gradient was exactly 0 and the kernel's cosine against it fell to 0.98)."""
 
     @staticmethod

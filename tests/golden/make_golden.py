@@ -1,13 +1,12 @@
-"""Generate golden vectors by importing the UNMODIFIED reference (/root/reference) on CPU.
+"""Generate golden vectors by importing the UNMODIFIED reference on CPU.
 
-Run once in the build container:  python tests/golden/make_golden.py
+Run once with a checkout of the reference:  NSR_REFERENCE_DIR=<checkout> python tests/golden/make_golden.py
 The reference cannot be imported as-is (tinycudann / nerfacc / pytorch_lightning / omegaconf ...
 are absent), so the third-party modules are stubbed in sys.modules; only the reference's own
 pure-torch code is executed: VanillaFrequency, VanillaMLP (incl. sphere-init + weight-norm and its
 autograd normal), CompositeEncoding, get_activation/trunc_exp, scale_anything,
 contract_to_unisphere, VarianceNetwork, NeuSModel.get_alpha, ray_utils.get_ray_directions/get_rays.
-Outputs: tests/golden/reference_torch.npz (small, committed).  /root/reference does not exist on
-the GPU box; tests only read the .npz.
+Outputs: tests/golden/reference_torch.npz (small, committed); tests only read the .npz.
 """
 import os
 import sys
@@ -17,7 +16,7 @@ import enum
 import numpy as np
 import torch
 
-REF = '/root/reference'
+REF = os.environ['NSR_REFERENCE_DIR']
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

@@ -1,8 +1,10 @@
 """Run in a subprocess by tests/test_reference_dropin.py.  Executes the UNMODIFIED reference training-step code -- ``preprocess_data`` and
 ``training_step`` of systems/nerf.py and systems/neus.py -- on the CPU with a tiny in-memory dataset and a fake model, and compares with
 the oracle restatements the GPU kernels are tested against: oracle/rays.py (pixel -> ray front end), oracle/losses.py (loss blocks,
-dynamic ray count).  Only packages that are not installed and not on the path (lightning, omegaconf, imaging libraries) are stubbed."""
-import contextlib
+dynamic ray count), and nsr_b200.optim.parse_optimizer with the reference's param groups.  The reference's side is replayed from
+tests/golden/reference_system.npz (tests/helpers/golden_ref.py: NSR_REFERENCE_DIR re-records it).  When recording, the reference's
+systems also drive the drop-in models through a few training steps ('integration'): that part is the reference's own driver code
+calling the product and only runs where a reference checkout is available."""
 import json
 import os
 import sys
@@ -12,47 +14,22 @@ import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-REF = '/root/reference'
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
-def _stub(name, **attrs):
-    m = types.ModuleType(name)
-    m.__dict__.update(attrs)
-    sys.modules[name] = m
-    return m
-
-
 def main():
     import cpu_thirdparty as tp
-    from nsr_b200.config import Config, to_primitive
+    import golden_ref
+    from nsr_b200.config import Config
     from oracle import rays as orays, losses as olosses
-    sys.modules['tinycudann'] = tp.tinycudann_module()
-    nerfacc, inter = tp.nerfacc_modules()
-    sys.modules['nerfacc'], sys.modules['nerfacc.intersection'] = nerfacc, inter
-    quiet = lambda *a, **k: None
-    rz = _stub('pytorch_lightning.utilities.rank_zero', rank_zero_info=quiet, rank_zero_debug=quiet, rank_zero_warn=quiet)
-    ut = _stub('pytorch_lightning.utilities', rank_zero=rz)
-    _stub('pytorch_lightning', utilities=ut, LightningModule=torch.nn.Module, LightningDataModule=object, Callback=object)
-    _stub('torch_efficient_distloss', flatten_eff_distloss=None)
-
-    class _OmegaConf:
-        @staticmethod
-        def register_new_resolver(*a, **k):
-            pass
-
-        @staticmethod
-        def to_container(c, resolve=True):
-            return to_primitive(c)
-    _stub('omegaconf', OmegaConf=_OmegaConf)
-    for name in ('imageio', 'cv2', 'trimesh', 'mcubes'):
-        _stub(name, marching_cubes=None)
-    mc, mp = _stub('matplotlib.colors', LinearSegmentedColormap=object), _stub('matplotlib.pyplot')
-    _stub('matplotlib', colors=mc, pyplot=mp, cm=types.SimpleNamespace())
-    torch.cuda.device = lambda idx: contextlib.nullcontext()
-    sys.path.insert(0, REF)
-    import systems as ref_systems          # the reference's systems package: nerf.py, neus.py, base.py, criterions.py, utils.py
+    R = golden_ref.Golden('reference_system')
+    if R.recording:
+        sys.modules['tinycudann'] = tp.tinycudann_module()
+        nerfacc, inter = tp.nerfacc_modules()
+        sys.modules['nerfacc'], sys.modules['nerfacc.intersection'] = nerfacc, inter
+        golden_ref.import_reference(stub_systems=False)
+        import systems as ref_systems          # the reference's systems package: nerf.py, neus.py, base.py, criterions.py, utils.py
 
     # ---- a tiny dataset in memory (what datasets/blender.py puts on the device)
     rng = np.random.default_rng(0)
@@ -94,37 +71,42 @@ def main():
     n_rays = 257
     model_cfg = dict(name='nerf', train_num_rays=n_rays, num_samples_per_ray=64, max_train_num_rays=1024, dynamic_ray_sampling=True,
                      batch_image_sampling=True, background_color='random')
-    s = make_system(ref_systems.systems['nerf-system'], model_cfg, dict(lambda_rgb=1.0, lambda_distortion=0.0))
     g = torch.Generator().manual_seed(3)
     out = {'comp_rgb': torch.rand(n_rays, 3, generator=g, requires_grad=True), 'rays_valid': torch.rand(n_rays, 1, generator=g) > 0.3,
            'num_samples': torch.tensor([9000], dtype=torch.int32)}
-    s.model = FakeModel(out)
-    torch.manual_seed(11)
-    batch = {}
-    s.preprocess_data(batch, 'train')
+
+    def nerf_reference():
+        s = make_system(ref_systems.systems['nerf-system'], model_cfg, dict(lambda_rgb=1.0, lambda_distortion=0.0))
+        s.model = FakeModel(out)
+        torch.manual_seed(11)
+        batch = {}
+        s.preprocess_data(batch, 'train')
+        loss = s.training_step(batch, 0)['loss']
+        loss.backward()
+        g_ref = out['comp_rgb'].grad.clone()
+        out['comp_rgb'].grad = None
+        bg_ref = s.model.background_color.clone()   # (the validation call below sets its own background)
+        vb = {'index': torch.tensor([2])}        # validation path: every pixel of one image (systems/nerf.py:57-64)
+        s.preprocess_data(vb, 'validation')
+        return {'rays': batch['rays'], 'rgb': batch['rgb'], 'fg_mask': batch['fg_mask'], 'bg': bg_ref, 'loss': float(loss.detach()),
+                'grad': g_ref, 'train_num_rays': s.train_num_rays, 'image_rays': vb['rays']}
+    ref = R('nerf', nerf_reference)
     torch.manual_seed(11)                  # the same draws, in the reference's order: index, x, y, then the random background colour
     index = torch.randint(0, n_img, size=(n_rays,))
     x = torch.randint(0, W, size=(n_rays,))
     y = torch.randint(0, H, size=(n_rays,))
     bg = torch.rand((3,))
     o_rays, o_rgb, o_fg = orays.training_batch(directions, c2w, images, masks, index.numpy(), x.numpy(), y.numpy(), bg=bg.numpy(), apply_mask=True)
-    loss = s.training_step(batch, 0)['loss']
-    loss.backward()
-    g_ref = out['comp_rgb'].grad.clone()
-    out['comp_rgb'].grad = None
     o_loss = olosses.nerf_loss(out, torch.from_numpy(o_rgb))
     o_loss.backward()
-    res['nerf'] = {'rays': float(np.abs(batch['rays'].numpy() - o_rays).max()), 'rgb': float(np.abs(batch['rgb'].numpy() - o_rgb).max()),
-                   'fg_mask': float(np.abs(batch['fg_mask'].numpy() - o_fg).max()),
-                   'bg_equal': bool(torch.equal(s.model.background_color, bg)),
-                   'loss': float(loss.detach()), 'loss_oracle': float(o_loss.detach()),
-                   'grad': float((g_ref - out['comp_rgb'].grad).abs().max()),
-                   'train_num_rays': s.train_num_rays,
-                   'train_num_rays_oracle': olosses.next_train_num_rays(n_rays, n_rays * 64, 9000, 1024)}
-    # validation path: every pixel of one image (systems/nerf.py:57-64)
-    vb = {'index': torch.tensor([2])}
-    s.preprocess_data(vb, 'validation')
-    res['nerf']['image_rays'] = float(np.abs(vb['rays'].numpy() - orays.image_batch(directions, c2w, 2)).max())
+    res['nerf'] = {'rays': float(np.abs(ref['rays'].numpy() - o_rays).max()), 'rgb': float(np.abs(ref['rgb'].numpy() - o_rgb).max()),
+                   'fg_mask': float(np.abs(ref['fg_mask'].numpy() - o_fg).max()),
+                   'bg_equal': bool(torch.equal(ref['bg'], bg)),
+                   'loss': ref['loss'], 'loss_oracle': float(o_loss.detach()),
+                   'grad': float((ref['grad'] - out['comp_rgb'].grad).abs().max()),
+                   'train_num_rays': ref['train_num_rays'],
+                   'train_num_rays_oracle': olosses.next_train_num_rays(n_rays, n_rays * 64, 9000, 1024),
+                   'image_rays': float(np.abs(ref['image_rays'].numpy() - orays.image_batch(directions, c2w, 2)).max())}
 
     # ---- NeuS system: training_step (systems/neus.py:91-153)
     k = 4000
@@ -132,30 +114,64 @@ def main():
                      batch_image_sampling=True, background_color='white', learned_background=False)
     lam = dict(lambda_rgb_mse=10.0, lambda_rgb_l1=0.7, lambda_mask=0.1, lambda_eikonal=0.1, lambda_curvature=0.0, lambda_sparsity=0.02,
                lambda_distortion=0.0, lambda_distortion_bg=0.0, lambda_opaque=0.05, sparsity_scale=3.0)
-    s = make_system(ref_systems.systems['neus-system'], model_cfg, lam)
     leaf = lambda *shape: torch.rand(*shape, generator=g).requires_grad_(True)
     out = {'comp_rgb_full': leaf(n_rays, 3), 'rays_valid_full': torch.rand(n_rays, 1, generator=g) > 0.3, 'opacity': leaf(n_rays, 1),
            'sdf_grad_samples': (torch.randn(k, 3, generator=g) * 1.3).requires_grad_(True),
            'sdf_samples': (torch.randn(k, generator=g) * 0.2).requires_grad_(True), 'num_samples_full': torch.tensor([5000], dtype=torch.int32),
            'inv_s': torch.tensor(20.0)}
-    s.model = FakeModel(out)
     batch = {'rays': torch.zeros(n_rays, 6), 'rgb': torch.rand(n_rays, 3, generator=g), 'fg_mask': (torch.rand(n_rays, generator=g) > 0.5).float()}
-    loss = s.training_step(batch, 0)['loss']
-    loss.backward()
     names = ('comp_rgb_full', 'opacity', 'sdf_grad_samples', 'sdf_samples')
-    g_ref = {n: out[n].grad.clone() for n in names}
-    for n in names:
-        out[n].grad = None
+
+    def neus_reference():
+        s = make_system(ref_systems.systems['neus-system'], model_cfg, lam)
+        s.model = FakeModel(out)
+        loss = s.training_step(batch, 0)['loss']
+        loss.backward()
+        g_ref = {n: out[n].grad.clone() for n in names}
+        for n in names:
+            out[n].grad = None
+        return {'loss': float(loss.detach()), 'grad': g_ref, 'train_num_rays': s.train_num_rays}
+    ref = R('neus', neus_reference)
     o_loss, terms = olosses.neus_loss(out, batch['rgb'], batch['fg_mask'],
                                       dict(rgb_mse=10.0, rgb_l1=0.7, eikonal=0.1, mask=0.1, opaque=0.05, sparsity=0.02, sparsity_scale=3.0))
     o_loss.backward()
-    res['neus'] = {'loss': float(loss.detach()), 'loss_oracle': float(o_loss.detach()),
-                   'grad': {n: float((g_ref[n] - out[n].grad).abs().max()) for n in names},
-                   'train_num_rays': s.train_num_rays,
+    res['neus'] = {'loss': ref['loss'], 'loss_oracle': float(o_loss.detach()),
+                   'grad': {n: float((ref['grad'][n] - out[n].grad).abs().max()) for n in names},
+                   'train_num_rays': ref['train_num_rays'],
                    'train_num_rays_oracle': olosses.next_train_num_rays(n_rays, n_rays * 64, 5000, 1024)}
     # ---- the reference's systems driving the DROP-IN models (INTEGRATION.md level 2), a few real training steps on the CPU: the models'
     # CUDA modules swapped for the stand-ins, everything else -- preprocess_data, update_module_step, training_step, the optimizer built by
     # the reference's parse_optimizer -- is the reference's own code calling our model classes
+    from nsr_b200 import models as our_models, configs
+    if R.recording:
+        integration(res, tp, ref_systems, make_system, dataset, lam, W, H)
+
+    # ---- parse_optimizer (systems/utils.py:314-325) on the same model and config section: param groups of the reference vs ours
+    from nsr_b200.optim import parse_optimizer
+    m = our_models.make('neus', configs.neus_dtu())
+    ocfg = dict(name='AdamW', args=dict(lr=0.01, betas=[0.9, 0.99], eps=1.e-15),
+                params=dict(geometry=dict(lr=0.01), texture=dict(lr=0.01), geometry_bg=dict(lr=0.01), texture_bg=dict(lr=0.01), variance=dict(lr=0.001)))
+    keys = ('lr', 'betas', 'eps', 'weight_decay')
+    pname = {id(p): n for n, p in m.named_parameters()}
+
+    def groups(opt):
+        return {'class': type(opt).__name__, 'names': [g_['name'] for g_ in opt.param_groups],
+                'hyper': [{k_: (list(g_[k_]) if isinstance(g_[k_], (list, tuple)) else g_[k_]) for k_ in keys} for g_ in opt.param_groups],
+                'params': [[pname[id(p)] for p in g_['params']] for g_ in opt.param_groups]}
+
+    def optimizer_reference():
+        from systems.utils import parse_optimizer as ref_parse_optimizer
+        return groups(ref_parse_optimizer(Config(ocfg), m))
+    ro, oo = R('optimizer', optimizer_reference), groups(parse_optimizer(Config(ocfg), m))
+    res['optimizer'] = {'ref_class': ro['class'], 'our_class': oo['class'], 'names_equal': ro['names'] == oo['names'],
+                        'hyper_equal': ro['hyper'] == oo['hyper'], 'same_tensors': ro['params'] == oo['params'], 'n_groups': len(oo['names'])}
+    R.save()
+    print('RESULT ' + json.dumps(res))
+
+
+def integration(res, tp, ref_systems, make_system, dataset, lam, W, H):
+    """the reference's systems driving the drop-in models: a few real training steps on the CPU (recording only)"""
+    from nsr_b200.config import Config
     from systems.utils import parse_optimizer as ref_parse_optimizer, update_module_step as ref_update_module_step
     from nsr_b200 import models as our_models, configs, tcnn as our_tcnn, nerfacc as our_nerfacc
     from nsr_b200.models import nerf_model, neus_model
@@ -237,22 +253,6 @@ def main():
                                     'val_psnr': float(vout['psnr']), 'val_index': int(vout['index'][0]), 'val_grid': grids[0][1],
                                     'mesh_name': meshes[0][0], 'mesh': meshes[0][1]}
 
-    # ---- parse_optimizer (systems/utils.py:314-325) on the same model and config section: param groups of the reference vs ours
-    from nsr_b200.optim import parse_optimizer
-    m = our_models.make('neus', configs.neus_dtu())
-    ocfg = dict(name='AdamW', args=dict(lr=0.01, betas=[0.9, 0.99], eps=1.e-15),
-                params=dict(geometry=dict(lr=0.01), texture=dict(lr=0.01), geometry_bg=dict(lr=0.01), texture_bg=dict(lr=0.01), variance=dict(lr=0.001)))
-    ro, oo = ref_parse_optimizer(Config(ocfg), m), parse_optimizer(Config(ocfg), m)
-    keys = ('lr', 'betas', 'eps', 'weight_decay')
-    res['optimizer'] = {
-        'ref_class': type(ro).__name__, 'our_class': type(oo).__name__,
-        'names_equal': [g_['name'] for g_ in ro.param_groups] == [g_['name'] for g_ in oo.param_groups],
-        'hyper_equal': all(tuple(a[k]) == tuple(b[k]) if isinstance(a[k], (list, tuple)) else a[k] == b[k]
-                           for a, b in zip(ro.param_groups, oo.param_groups) for k in keys),
-        'same_tensors': all(len(a['params']) == len(b['params']) and all(x is y for x, y in zip(a['params'], b['params']))
-                            for a, b in zip(ro.param_groups, oo.param_groups)),
-        'n_groups': len(oo.param_groups)}
-    print('RESULT ' + json.dumps(res))
 
 
 if __name__ == '__main__':

@@ -1,4 +1,4 @@
-"""GPU tests that have not run on a B200 yet are at least dry-run here: their whole logic (fixtures, oracle side, tolerances, output keys)
+"""GPU tests are at least dry-run here: their whole logic (fixtures, oracle side, tolerances, output keys)
 and the models' Python paths execute on the CPU with the oracle-backed stand-ins in place of the CUDA modules
 (tests/helpers/dryrun_gpu_tests.py).  What is left for the GPU box is the kernels, each of which has its own parity test."""
 import os

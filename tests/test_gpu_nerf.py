@@ -63,7 +63,7 @@ def oracle_run(model, binary, rays, jitter, bg, target):
 @pytest.mark.parametrize('fused', ['per_ray', 'per_ray_split', 'per_ray_tc', 'per_ray_bwd', 'two_pass', False])
 def test_nerf_model_forward_backward_parity(fused):
     """per_ray: per-ray forward kernel + tile backward; per_ray_split: the tile backward as network half + table-scatter half;
-    per_ray_tc: the tcgen05 / TMA backward (csrc/nerf_bwd_tc.cu);
+    per_ray_tc: the wgmma / TMA backward (csrc/nerf_bwd_tc.cu);
     per_ray_bwd: per-ray forward AND backward kernels;
     two_pass: pre-pass + sample-tile kernels; False: per-op composition"""
     check_parity(fused, 600)

@@ -57,7 +57,7 @@ def test_neus_blender_forward_backward_parity():
 
 def test_neus_full_size_c3_8192_rays_parity():
     """BASELINE.json config 3 at its full size (neus-blender with mask, 8192 rays; 183,584 samples on the synthetic occupancy with these
-    seeds, measured on B200 = the oracle's count): same tolerances as the 300-ray case."""
+    seeds = the oracle's count): same tolerances as the 300-ray case."""
     check_neus_blender(8192, 7, 150000)
 
 

@@ -391,7 +391,7 @@ def test_occupancy_grid_update(nsr):
 
 @pytest.mark.parametrize('n_in,n_out,nh,oact', [(32, 16, 1, 'None'), (32, 3, 2, 'Sigmoid'), (64, 4, 2, 'None'), (16, 1, 3, 'None')])
 def test_mlp_fwd_tcgen05_matches_mma_sync(nsr, n_in, n_out, nh, oact):
-    """nsr_mlp_fwd_tc (tcgen05.mma + TMEM) computes the same network as nsr_mlp_fwd (mma.sync) and as the oracle."""
+    """nsr_mlp_fwd_tc (wgmma.mma_async) computes the same network as nsr_mlp_fwd (mma.sync) and as the oracle."""
     nsr_b200, ops, tcnn, _ = nsr
     from nsr_b200.lib import lib, ptr, stream
     D = dev()
@@ -411,8 +411,8 @@ def test_mlp_fwd_tcgen05_matches_mma_sync(nsr, n_in, n_out, nh, oact):
     assert (got - ref).abs().max().item() <= 2e-3 * max(1.0, ref.abs().max().item())
     yr = omlp.ffmlp_fwd(x.float().cpu(), net.params.detach().cpu(), n_in, n_out, 64, nh, 'ReLU', oact, emulate_fp16=True)
     assert (got.cpu() - yr).abs().max().item() <= 2e-2 * yr.abs().max().item() + 2e-3
-    # the module-level switch: tcnn.Network(..., {'backend': 'tcgen05'}) routes the forward through the same kernel, autograd intact
-    net_tc = tcnn.Network(n_in, n_out, dict(cfg, backend='tcgen05')).to(D)
+    # the module-level switch: tcnn.Network(..., {'backend': 'wgmma'}) routes the forward through the same kernel, autograd intact
+    net_tc = tcnn.Network(n_in, n_out, dict(cfg, backend='wgmma')).to(D)
     with torch.no_grad():
         net_tc.params.copy_(net.params)
     xg = x.float().requires_grad_(True)

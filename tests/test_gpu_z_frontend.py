@@ -3,8 +3,7 @@ oracle/rays.py (numpy fp32 restatement of systems/nerf.py:33-91 + models/ray_uti
 Tolerance: origins, colours, masks exact (copies; the mask blend is three fp32 ops in the reference's order); directions 2e-7 absolute
 (the order of the 3-term sums inside torch is not specified).
 
-Seen on a B200 in profiles/r1_experimental_gpu_tests.log (every comparison below held; the only failure there was the n = 0 call at the
-end of the first test, since made an early return)."""
+The n = 0 call at the end of the first test is an early return."""
 import numpy as np
 import pytest
 import torch

@@ -2,8 +2,7 @@
 oracle's render + torch.optim.AdamW (the reference's optimizer, systems/utils.py:314-325) from identical parameters, rays, jitter and
 targets.  Adam normalises every gradient entry, so table entries whose gradient is rounding noise may step differently; the loss is what
 must agree.  Tolerance: per-step loss within 3 % of the oracle's for six steps, and the loss must go down on both sides.
-
-First seen green on a B200 in round 2 (profiles/r2_gputest_first.log)."""
+"""
 import os
 
 import numpy as np

@@ -5,7 +5,7 @@ reference's own torch fields (optionally on the fused VanillaMLP kernels), again
 Tolerances: kept-sample counts equal up to samples whose transmittance sits at early_stop_eps (<= 3), per-ray colour 2e-3 (5e-3 with the
 fp16-operand VanillaMLP kernels), network gradients cosine >= 0.999 (0.99).
 
-First seen green on a B200 in round 2 (profiles/r2_gputest_first.log); runs un-gated."""
+Runs un-gated."""
 import os
 
 import numpy as np

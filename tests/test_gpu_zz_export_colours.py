@@ -1,7 +1,7 @@
 """Vertex-colour export (models/neus.py:321-329, models/nerf.py:153-161) through the drop-in models on the GPU: isosurface by the GPU
 marching cubes, per-vertex features through the fused SDF field / colour kernels.  Every kernel on this path has its own parity test; the
 Python path (chunk_batch keyword arguments, eval-mode detaching, the texture call with the normal as view direction) was dry-run on the
-CPU with the oracle-backed stand-ins (tests/test_dryrun.py).  First seen green on a B200 in round 2 (profiles/r2_gputest_first.log)."""
+CPU with the oracle-backed stand-ins (tests/test_dryrun.py)."""
 import os
 
 import pytest

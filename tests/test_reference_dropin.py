@@ -1,7 +1,9 @@
-"""Drop-in check at INTEGRATION.md level 1: the UNMODIFIED reference models (/root/reference/models/*.py) import ``tinycudann`` and
-``nerfacc`` and get nsr_b200's modules; they construct with the reference's own configs, expose the parameter counts SURVEY.md 8a
-states, share state_dict keys / shapes with the drop-in models (checkpoints load both ways) and refuse CPU tensors the way
-nerfacc 0.3.3 / tiny-cuda-nn do.  Needs /root/reference (present in the build container, absent on the GPU box => skipped there)."""
+"""Drop-in check at INTEGRATION.md level 1 and the pins of the oracle to the reference's own code.  Each helper compares the product or
+the oracle with what the UNMODIFIED reference computes; the reference's side is stored under tests/golden/ (recorded from a checkout of
+the reference with NSR_REFERENCE_DIR set, see tests/helpers/golden_ref.py) and replayed here, so these tests run everywhere.  The
+reference models import ``tinycudann`` and ``nerfacc`` and get nsr_b200's modules; they construct with the reference's own configs,
+expose the parameter counts SURVEY.md 8a states, share state_dict keys / shapes with the drop-in models (checkpoints load both ways) and
+refuse CPU tensors the way nerfacc 0.3.3 / tiny-cuda-nn do."""
 import json
 import os
 import subprocess
@@ -12,7 +14,6 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/models'), reason='/root/reference is not mounted here')
 def test_reference_models_build_on_our_modules():
     r = subprocess.run([sys.executable, os.path.join(ROOT, 'tests', 'helpers', 'reference_dropin.py')], capture_output=True, text=True,
                        timeout=600)
@@ -29,12 +30,12 @@ def test_reference_models_build_on_our_modules():
         assert e['keys_equal'] and e['shapes_equal'] and not e['only_ref'] and not e['only_ours'], e
         assert e['cpu_forward'] == 'NotImplementedError'
         assert e['grid_is_ours'] == 'nsr_b200.nerfacc'
+        assert e['loads_ref'] and e['loads_ours']
     assert nerf['tcnn_modules'] == ['Encoding', 'Network', 'NetworkWithInputEncoding']
     assert neus['tcnn_modules'] == ['Encoding', 'Network']
     assert dtu['n_params'] == dtu['n_params_ours'] and dtu['tcnn_modules'] == ['Encoding']  # neus-dtu: VanillaMLPs everywhere
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/models'), reason='/root/reference is not mounted here')
 def test_oracle_orchestration_is_pinned_to_the_reference_forward():
     """oracle/models.py (nerf_render, neus_render, neus_bg_render, neus_dtu_render) restates models/nerf.py:61-127 and models/neus.py:141-287.  Here the reference's
     OWN forward_ runs on the CPU -- tinycudann / nerfacc replaced by per-op stand-ins built from the oracle's primitives
@@ -70,7 +71,6 @@ def test_oracle_orchestration_is_pinned_to_the_reference_forward():
     assert dtu['occ_fn_bg'] < 1e-6 and dtu['occ_thre'] == [0.001, 0.01]       # the background grid keeps the default threshold
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/systems'), reason='/root/reference is not mounted here')
 def test_oracle_front_end_and_losses_are_pinned_to_the_reference_training_step():
     """The reference's OWN systems/nerf.py / systems/neus.py ``preprocess_data`` and ``training_step`` run on the CPU (tiny in-memory
     dataset, fake model; tests/helpers/reference_system.py): the batch they assemble equals oracle.rays.training_batch / image_batch (the
@@ -88,8 +88,10 @@ def test_oracle_front_end_and_losses_are_pinned_to_the_reference_training_step()
     assert abs(neus['loss'] - neus['loss_oracle']) < 1e-6 and max(neus['grad'].values()) < 1e-7
     assert neus['train_num_rays'] == neus['train_num_rays_oracle'] == RayBudget.rule(257, 257 * 64, 5000, 1024)
     # level 2: the reference's systems (preprocess_data, update_module_step, training_step, parse_optimizer) drive OUR model classes for a
-    # few real optimizer steps on the CPU (CUDA modules swapped for the stand-ins): it trains, and the ray budget reacts
-    for kind in ('nerf', 'neus'):
+    # few real optimizer steps on the CPU (CUDA modules swapped for the stand-ins): it trains, and the ray budget reacts.  This is the
+    # reference's driver code executing, so it runs only where a reference checkout is given (NSR_REFERENCE_DIR); without one, the
+    # product's own training loop over the same models is covered by test_abi_and_host.py::test_train_synthetic_tool_logic_runs_on_cpu_standins
+    for kind in (('nerf', 'neus') if 'integration' in res else ()):
         e = res['integration'][kind]
         assert e['model_class'] == f'nsr_b200.models.{kind}_model' and len(e['losses']) == 4
         assert e['losses'][-1] < e['losses'][0] and all(v == v for v in e['losses'])
@@ -106,7 +108,6 @@ def test_oracle_front_end_and_losses_are_pinned_to_the_reference_training_step()
     assert opt['names_equal'] and opt['hyper_equal'] and opt['same_tensors']
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/models'), reason='/root/reference is not mounted here')
 def test_product_torch_side_equals_the_reference_functions():
     """every pure-torch piece of the drop-in models compared DIRECTLY with the reference's own (tests/helpers/reference_torch_parts.py):
     activations (value + gradient), scale_anything, contraction, chunk_batch, VanillaFrequency mask schedule, VanillaMLP / tcnn sphere
@@ -127,7 +128,6 @@ def test_product_torch_side_equals_the_reference_functions():
         assert worst(section) == 0.0, (name, section)
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/models'), reason='/root/reference is not mounted here')
 def test_product_volume_sdf_torch_paths_equal_the_reference():
     """VolumeSDF paths of the product that are torch code rather than kernels -- finite-difference normals + laplacian under the
     ProgressiveBandHashGrid schedule (configs/neuralangelo-dtu-wmask.yaml), fixed-eps finite differences, the autograd fallback of the
@@ -147,7 +147,6 @@ def test_product_volume_sdf_torch_paths_equal_the_reference():
                 assert v <= tol, (section, case, name, v)
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/models'), reason='/root/reference is not mounted here')
 def test_product_models_composed_path_equals_the_reference_models_on_cpu():
     """The drop-in 'nerf' / 'neus' models run their per-op (composed) code path on the CPU -- tcnn modules swapped for the oracle-backed
     stand-ins, nerfacc-shaped functions rebound to them (tests/helpers/reference_product_composed.py) -- against the unmodified reference

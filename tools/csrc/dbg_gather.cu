@@ -164,9 +164,9 @@ __global__ void __launch_bounds__(256) dbg_scatter_kernel(const __grid_constant_
 }
 
 
-// ---- round 2: warp-wide run merging + paired 16-byte REDs, thread per sample (what the scatter warps of the tcgen05 backward do) -------
+// ---- warp-wide run merging + paired 16-byte REDs, thread per sample (what the scatter warps of the tensor-core backward do) -------
 // lanes = 32 consecutive samples (ray-major order); on levels < MERGE_LEVELS runs of equal cells are summed with a segmented shuffle
-// scan over the WHOLE warp (round 1 merged over 8 lanes) and only the run's last lane issues REDs; x-adjacent corners that are
+// scan over the WHOLE warp and only the run's last lane issues REDs; x-adjacent corners that are
 // neighbours in memory go out as one red.v4.f32.  PAIR = 0: 8-byte REDs only.
 template <int MERGE_LEVELS, int PAIR>
 __global__ void __launch_bounds__(256) dbg_scatter_merged_kernel(const __grid_constant__ nsr_grid_t g, const float* __restrict__ pos,

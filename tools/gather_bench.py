@@ -84,7 +84,7 @@ for variant in (0, 1, 2, 3, 4, 5):
         assert (grad - ref_grad).abs().max().item() <= 1e-3 * ref_grad.abs().max().item(), 'v5 mismatch'
 print(json.dumps(sres))
 
-# ---- round 2: warp-wide run merging (+ paired 16-byte REDs), thread per sample, occupancy sweep
+# ---- warp-wide run merging (+ paired 16-byte REDs), thread per sample, occupancy sweep
 mres = {'k': k}
 for ml in (0, 6, 8, 10):
     for pair in (0, 1):

@@ -1,5 +1,5 @@
 """Timing of the drop-in 'neus' model (configs C3 neus-blender 8192 rays, C4 neus-dtu 4096 rays + learned background) on the
-per-op CUDA surface: forward + reference losses (systems/neus.py:98-113) + backward.  Development / profiles aid."""
+per-op CUDA surface: forward + reference losses (systems/neus.py:98-113) + backward.  Development aid."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch, torch.nn.functional as F

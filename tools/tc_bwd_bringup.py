@@ -1,4 +1,4 @@
-"""Bring-up of the tcgen05 backward (nsr_nerf_field_bwd_tc) on the bench workload: one eager step per backward kernel ('tiles' = the
+"""Bring-up of the wgmma backward (nsr_nerf_field_bwd_tc) on the bench workload: one eager step per backward kernel ('tiles' = the
 mma.sync tile kernel, 'tiles_split', 'tc'), gradients compared with the 'tiles' result, kernel times from CUDA events around the C-ABI calls."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
