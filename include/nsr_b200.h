@@ -255,7 +255,9 @@ int nsr_nerf_field_bwd_split(const nsr_nerf_t* f, const void* enc_k_h, const voi
                              const int64_t* k_dev, const float* xyzdir, void* denc_h, void* stream);
 /* The two halves of nsr_nerf_field_bwd_split as separate calls (same arguments; the split form = net followed by scatter with
  * xyz = xyzdir, stride = 6, grad_table = grad_dparams + 3072 = the density network's parameter count, levels [0, 16), ctas_per_sm 0 = 8).
- * The data-parallel step scatters level groups in separate launches so that the exchange of a finished group overlaps the next group.  autograd of tcnn's
+ * denc_h must be 8-byte aligned.  The fused backward scatters level groups in separate launches and zeroes each group's slice of the table
+ * right before its launch, so that the slice the REDs hit stays in L2; the data-parallel step also exchanges a finished group beside the
+ * next group's scatter.  autograd of tcnn's
  * NetworkWithInputEncoding / Network (models/geometry.py:122-130, models/texture.py:23-30): network half, then the grid backward. */
 int nsr_nerf_field_bwd_net(const nsr_nerf_t* f, const void* enc_k_h, const void* dparams_h, const void* cparams_h, const float* d_sraw,
                            const float* d_rgb, float* grad_dparams, float* grad_cparams, float loss_scale, const float* amax, int64_t k,

@@ -413,11 +413,14 @@ __global__ void __launch_bounds__(256, MINB) nerf_table_scatter_kernel(const __g
       y = xyz[i * stride + 1];
       z = xyz[i * stride + 2];
     }
+    uint2 dq = make_uint2(0u, 0u);   // the row's d(encoding) of the level pair that holds level l: one 8-byte load per pair
 #pragma unroll 1
-    for (int l = l_begin; l < l_end; ++l) {  // the data-parallel step scatters level groups in separate launches (gradient exchange overlap)
+    for (int l = l_begin; l < l_end; ++l) {  // the backward scatters level groups in separate launches (each group's gradient slice stays in L2)
       float2 d = make_float2(0.f, 0.f);
       if (ok) {
-        d = __half22float2(denc[i * 16 + l]);
+        if (l == l_begin || (l & 1) == 0) dq = __ldg(reinterpret_cast<const uint2*>(denc + i * 16 + (l & ~1)));
+        const uint32_t h = (l & 1) ? dq.y : dq.x;
+        d = __half22float2(*reinterpret_cast<const __half2*>(&h));
         d.x *= inv_scale;
         d.y *= inv_scale;
       }
@@ -538,6 +541,7 @@ extern "C" int nsr_nerf_table_scatter(const nsr_grid_t* g, const float* xyz, int
   NSR_REQUIRE(g->n_levels == 16 && g->n_features == 2, "nsr_nerf_table_scatter: needs L=16, F=2");
   NSR_REQUIRE(loss_scale > 0.f || amax != nullptr, "nsr_nerf_table_scatter: loss_scale <= 0 (automatic) needs the amax pointer");
   NSR_REQUIRE(stride >= 3, "nsr_nerf_table_scatter: stride must be >= 3");
+  NSR_REQUIRE((uintptr_t)denc_h % 8 == 0, "nsr_nerf_table_scatter: denc must be 8-byte aligned");
   NSR_REQUIRE(level_begin >= 0 && level_begin <= level_end && level_end <= 16, "nsr_nerf_table_scatter: bad level range [%d, %d)", level_begin, level_end);
   if (k == 0 || level_begin == level_end) return 0;
   const int per_sm = ctas_per_sm >= 1 && ctas_per_sm <= 8 ? ctas_per_sm : 8;   // < 8 leaves room for a kernel running beside it (the exchange)
@@ -566,6 +570,7 @@ extern "C" int nsr_nerf_field_bwd_split(const nsr_nerf_t* f, const void* enc_k_h
                                         const float* d_sraw, const float* d_rgb, float* grad_dparams, float* grad_cparams, float loss_scale,
                                         const float* amax, int64_t k, const int64_t* k_dev, const float* xyzdir, void* denc_h, void* stream) {
   NSR_REQUIRE(denc_h != nullptr && xyzdir != nullptr, "nsr_nerf_field_bwd_split: denc / xyzdir is NULL");
+  NSR_REQUIRE((uintptr_t)denc_h % 8 == 0, "nsr_nerf_field_bwd_split: denc must be 8-byte aligned");
   const int rc = field_bwd_launch(f, nullptr, nullptr, nullptr, nullptr, enc_k_h, dparams_h, cparams_h, d_sraw, d_rgb, grad_dparams, grad_cparams,
                                   loss_scale, amax, k, k_dev, nullptr, xyzdir, denc_h, stream, "nsr_nerf_field_bwd_split");
   if (rc != 0 || k == 0) return rc;

@@ -19,6 +19,11 @@ from . import ops
 from .lib import lib, ptr, stream, check_cuda, contig, NerfT
 from .nerfacc import ContractionType
 
+# Level groups of the split backward's table scatter, one launch each (top levels first).  Each group's slice of the fp32 table gradient
+# (16.5-16.8 MB here) is zeroed right in front of its launch and stays in the H100's 50 MB L2 while the REDs land on it; the whole
+# table (50 MB) does not.  Chosen with tools/scatter_bench.py.
+SCATTER_LEVEL_GROUPS = ((12, 16), (8, 12), (0, 8))
+
 
 class _NerfRender(torch.autograd.Function):
     """(dparams, cparams) -> per-ray sums + per-sample weights; everything else rides along non-differentiably."""
@@ -91,23 +96,6 @@ class _NerfRenderRays(torch.autograd.Function):
         i64 = lambda k: torch.empty(k, dtype=torch.int64, device=dev)
         words = (fused.cap_per_ray + 31) // 32
         need_grad = (dparams.requires_grad or cparams.requires_grad) and fused._want_grad   # (grad mode is always off inside Function.forward)
-        # The backward accumulates into zeroed flat gradient buffers (50 MB for the table).  Zero them NOW on a side stream: the fill runs
-        # beside the marcher / forward kernels instead of in front of the backward's first kernel; the backward joins the side stream.
-        ctx.grad_bufs = None
-        if need_grad and fused.prezero_grads:
-            cur = torch.cuda.current_stream()
-            side = fused.side_stream(dev)
-            if fused.direct_grads is not None:
-                gd0, gc0 = fused.direct_grads
-            else:
-                gd0, gc0 = torch.empty(fused.n_dparams, device=dev), torch.empty(fused.n_cparams, device=dev)
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                gd0.zero_()
-                gc0.zero_()
-            gd0.record_stream(side)
-            gc0.record_stream(side)
-            ctx.grad_bufs = (gd0, gc0, side)
         masks, t_min, counts = i32(n * words), f32(n), i32(n)
         # one fill: the forward's ray ticket, the backward's gradient amax, the marcher's row allocator and its 8 queue-group counters
         nb = (n + 255) // 256
@@ -167,17 +155,17 @@ class _NerfRenderRays(torch.autograd.Function):
         n, cap = ctx.n_rays, ctx.cap
         step = float(fused.model.render_step_size)
         direct = fused.direct_grads
-        pre, ctx.grad_bufs = getattr(ctx, 'grad_bufs', None), None   # (a retained-graph second backward allocates fresh buffers below)
-        if pre is not None and (direct is None or pre[0] is direct[0]):
-            gd, gc, side = pre                     # zeroed on the side stream while the forward ran
-            torch.cuda.current_stream().wait_stream(side)
-        elif direct is not None:   # accumulate straight into caller-owned buffers (the symmetric exchange buffer): autograd is bypassed
+        if direct is not None:   # accumulate straight into caller-owned buffers (the symmetric exchange buffer): autograd is bypassed
             gd, gc = direct
-            gd.zero_()
-            gc.zero_()
         else:
-            gd = torch.zeros(fused.n_dparams, device=dev)
-            gc = torch.zeros(fused.n_cparams, device=dev)
+            gd = torch.empty(fused.n_dparams, device=dev)
+            gc = torch.empty(fused.n_cparams, device=dev)
+        # The split backward zeroes the table gradient one level-group slice at a time, right in front of that group's scatter, so the
+        # slice its REDs hit is still in L2; here only the density network's weight gradients.  Every other form zeroes everything now.
+        n_head = fused.net.mlp.n_params
+        split = fused.bwd_kernel == 'tiles_split' and enc_k is not None and n > 0
+        (gd[:n_head] if split else gd).zero_()
+        gc.zero_()
         if (enc is not None or enc_k is not None) and n > 0:
             f32 = lambda t: None if t is None else contig(t, torch.float32)
             amax = amax0   # zeroed together with the forward's ticket (a retained-graph second backward only makes the scale smaller)
@@ -205,12 +193,17 @@ class _NerfRenderRays(torch.autograd.Function):
                     denc = torch.empty(cap, 32, dtype=torch.float16, device=dev)
                     lib.call('nsr_nerf_field_bwd_net', fused.ref(), ptr(enc_k), ptr(dh), ptr(ch), ptr(d_sraw), ptr(d_rgb), ptr(gd), ptr(gc),
                              float(fused.loss_scale), ptr(amax), cap, ptr(offsets_k[n:]), ptr(xyzdir), ptr(denc), stream())
-                    # table half; data-parallel runs scatter level groups in separate launches and hand each finished group to the gradient
-                    # exchange (parallel.P2PGradSync.bind_pipelined), whose kernel runs beside the next group's scatter (which leaves it one CTA slot per SM)
-                    groups = fused.level_groups or ((0, 16),)
+                    # table half, one launch per level group behind a fill of that group's slice: the 50 MB table gradient does not fit the
+                    # L2, one group's slice does.  Data-parallel runs hand each finished group to the gradient exchange
+                    # (parallel.P2PGradSync.bind_pipelined), whose kernel runs beside the next group's scatter (which leaves it one CTA slot per SM)
+                    groups = fused.level_groups or SCATTER_LEVEL_GROUPS
+                    off = fused.grid.offset
+                    if sorted(l for g in groups for l in range(*g)) != list(range(len(off) - 1)):
+                        raise ValueError(f'level_groups {groups} must partition the {len(off) - 1} levels: the backward zeroes the table per group')
                     for gi, (l0, l1) in enumerate(groups):
+                        gd[n_head + 2 * int(off[l0]):n_head + 2 * int(off[l1])].zero_()
                         lib.call('nsr_nerf_table_scatter', ctypes.byref(fused.struct.grid), ptr(xyzdir), 6, ptr(denc), float(fused.loss_scale), ptr(amax),
-                                 ptr(gd[fused.net.mlp.n_params:]), cap, ptr(offsets_k[n:]), l0, l1, 4 if (fused.exchange_hook is not None and gi > 0) else 0,
+                                 ptr(gd[n_head:]), cap, ptr(offsets_k[n:]), l0, l1, 4 if (fused.exchange_hook is not None and gi > 0) else 0,
                                  stream())
                         if fused.exchange_hook is not None:
                             fused.exchange_hook(gi)
@@ -262,12 +255,10 @@ class NerfFused:
         # the marcher allocates every ray's rows and queue slot itself (nsr_march_rays_alloc) instead of a one-CTA scan kernel behind it
         self.march_alloc = os.environ.get('NSR_MARCH_ALLOC', '1') == '1'
         self.direct_grads = None
-        # zero the backward's gradient buffers beside the forward on a side stream instead of in front of the backward: opt-in, because
-        # the fill kernel takes SMs from the persistent forward kernel at its launch.
-        self.prezero_grads = os.environ.get('NSR_PREZERO_GRADS', '0') == '1'
-        self._side = None
         self._want_grad = True
-        self.level_groups = None    # ((l0, l1), ...): the split backward's table scatter as one launch per level group (top levels first)
+        # ((l0, l1), ...) partitioning the levels: the split backward's table scatter as one launch per level group (top levels first);
+        # None = SCATTER_LEVEL_GROUPS
+        self.level_groups = None
         self.exchange_hook = None   # callable(group index): called behind each group's scatter launch (the gradient exchange of that group)
         self.t_bound = 16.0     # bound on the ray parameter t for the loss-scale estimate (depth gradient term)
 
@@ -299,11 +290,6 @@ class NerfFused:
 
     def ref(self):
         return ctypes.byref(self.struct)
-
-    def side_stream(self, dev):
-        if self._side is None or self._side.device != dev:
-            self._side = torch.cuda.Stream(device=dev)
-        return self._side
 
     def ticket(self, dev):
         if self._ticket is None or self._ticket.device != dev:
