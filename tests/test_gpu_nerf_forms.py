@@ -40,3 +40,23 @@ def test_allocating_marcher_and_level_group_scatter_equal_the_plain_forms():
     assert torch.equal(a['comp_rgb'], c['comp_rgb'])
     assert cos(gd_a, gd_c) >= 0.999999 and (gd_a - gd_c).abs().max().item() <= 1e-4 * gd_a.abs().max().item()
     assert torch.equal(gc_a, gc_c) or cos(gc_a, gc_c) >= 0.999999
+
+
+@pytest.mark.parametrize('n_rays,peak', [(1500, 10.0), (8192, None)])
+def test_unpacked_field_backward_equals_packed(n_rays, peak):
+    """packed_bwd_inputs = False: nsr_nerf_field_bwd reads the per-ray (loose) encodings and gradients through row_pos and recomputes the
+    sample positions from the rays; same gradients as the packed inputs up to the order of the fp32 atomics"""
+    model, cfg, binary, rays, jitter, bg = build('per_ray', n_rays=n_rays, seed=23, **({} if peak is None else {'peak': peak}))
+    target = torch.rand(len(rays), 3, generator=torch.Generator().manual_seed(6))
+    f = model._fused
+    assert f.bwd_kernel == 'tiles' and f.packed_bwd_inputs
+    a, gd_a, gc_a = _run(model, rays, jitter, target)
+    f.packed_bwd_inputs = False
+    try:
+        b, gd_b, gc_b = _run(model, rays, jitter, target)
+    finally:
+        f.packed_bwd_inputs = True
+    assert int(a['num_samples']) == int(b['num_samples']) > 20000
+    assert torch.equal(a['comp_rgb'], b['comp_rgb'])
+    for x, y in ((gd_a, gd_b), (gc_a, gc_b)):
+        assert cos(x, y) >= 0.999999 and (x - y).abs().max().item() <= 1e-4 * y.abs().max().item()
