@@ -470,6 +470,16 @@ int nsr_neus_loss_bwd(const nsr_neus_loss_t* p, const float* comp_rgb, const uin
                       const float* fg_mask, const float* sdf_grad, const float* sdf, const float* accum8, const float* g_loss,
                       float* g_comp_rgb, float* g_opacity, float* g_sdf_grad, float* g_sdf, int64_t n_rays, int64_t k, const int64_t* k_dev,
                       void* stream);
+/* Distortion loss of mip-NeRF 360 (torch_efficient_distloss.flatten_eff_distloss; systems/nerf.py:103-106, systems/neus.py:131-139) over
+ * n packed samples sorted by ray: loss = sum_rays [sum_ij w_i w_j |m_i - m_j| + 1/3 sum_i w_i^2 d_i] / (ray_ids[last live row] + 1).
+ * w_pos (int64 [n], may be NULL): the weight of row i is w[w_pos[i]] and its gradient goes to g_w[w_pos[i]].  t_mode 0: a = midpoints,
+ * b = intervals; t_mode 1: a = t_starts, b = t_ends.  n_dev (device int64, may be NULL): live row count; rows at or past it are never
+ * read or written.  fwd: accum2 = device float[2], zeroed here; [1] = the loss (0 for no live rows).  bwd: g_w at every live row =
+ * *g_loss (NULL = 1) * dloss/dw, plain stores (no other entry of g_w is written).  Neither synchronises with the host. */
+int nsr_distortion_fwd(const float* w, const int64_t* w_pos, const float* a, const float* b, int32_t t_mode, const int32_t* ray_ids,
+                       float* accum2, int64_t n, const int64_t* n_dev, void* stream);
+int nsr_distortion_bwd(const float* w, const int64_t* w_pos, const float* a, const float* b, int32_t t_mode, const int32_t* ray_ids,
+                       const float* g_loss, float* g_w, int64_t n, const int64_t* n_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -132,6 +132,8 @@ _SIGNATURES = {
     'nsr_nerf_field_bwd_net': [P, P, P, P, P, P, P, P, F32, P, I64, P, P, P, P],
     'nsr_nerf_table_scatter': [P, P, I32, P, F32, P, P, I64, P, I32, I32, I32, P],
     'nsr_nerf_field_bwd_tc': [P, P, P, P, P, P, P, P, F32, P, I64, P, P, P, P],
+    'nsr_distortion_fwd': [P, P, P, P, I32, P, P, I64, P, P],
+    'nsr_distortion_bwd': [P, P, P, P, I32, P, P, P, I64, P, P],
 }
 
 
@@ -189,7 +191,7 @@ lib = _Lib()
 
 
 # entry points that launch more than one kernel (lib.launches counts kernels, not calls)
-_KERNELS_PER_CALL = {'nsr_nerf_field_bwd_split': 2, 'nsr_nerf_loss_fwd': 2, 'nsr_neus_loss_fwd': 2, 'nsr_occgrid_update': 2, 'nsr_mc_count': 2, 'nsr_mc_emit': 2}
+_KERNELS_PER_CALL = {'nsr_nerf_field_bwd_split': 2, 'nsr_nerf_loss_fwd': 2, 'nsr_neus_loss_fwd': 2, 'nsr_distortion_fwd': 2, 'nsr_occgrid_update': 2, 'nsr_mc_count': 2, 'nsr_mc_emit': 2}
 
 
 def register_signatures(sigs):

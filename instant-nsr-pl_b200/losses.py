@@ -76,7 +76,7 @@ def neus_losses(out, rgb, fg_mask=None, lambda_rgb_mse=10.0, lambda_rgb_l1=0.0, 
     sdf_samples; plus 'num_samples_dev' -- the device-side live sample count -- when the model ran in static-shape mode);
     ``rgb`` [N,3] target, ``fg_mask`` [N] (None = dataset without masks).  Defaults = configs/neus-blender.yaml:80-89.
     -> (total, parts) with parts[i] = the un-weighted loss NEUS_LOSS_NAMES[i] (for logging).  curvature / distortion terms
-    (lambda 0 in every shipped config) stay with the caller."""
+    (lambda 0 in every shipped NeuS config) stay with the caller; the distortion term is ``distortion_loss`` below."""
     comp, op = out['comp_rgb_full'], out['opacity']
     check_cuda(comp, op, rgb, what='neus_losses')
     d = NeusLossT(float(lambda_rgb_mse), float(lambda_rgb_l1), float(lambda_eikonal), float(lambda_mask if fg_mask is not None else 0.0),
@@ -87,3 +87,71 @@ def neus_losses(out, rgb, fg_mask=None, lambda_rgb_mse=10.0, lambda_rgb_l1=0.0, 
                              None if fg_mask is None else contig(fg_mask.reshape(-1), torch.float32),
                              None if sg is None else contig(sg.reshape(-1, 3), torch.float32),
                              None if s is None else contig(s.reshape(-1), torch.float32), out.get('num_samples_dev'))
+
+
+class _Distortion(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, w, w_pos, a, b, t_mode, ray_ids, n_dev):
+        n = ray_ids.shape[0]
+        accum = torch.empty(2, device=w.device)   # zeroed by the entry point; [1] = the loss
+        lib.call('nsr_distortion_fwd', ptr(w), ptr(w_pos), ptr(a), ptr(b), t_mode, ptr(ray_ids), ptr(accum), n, ptr(n_dev), stream())
+        ctx.t_mode = t_mode
+        ctx.save_for_backward(w, w_pos, a, b, ray_ids, n_dev)
+        return accum[1]
+
+    @staticmethod
+    def backward(ctx, g_loss):
+        w, w_pos, a, b, ray_ids, n_dev = ctx.saved_tensors
+        # every live row (its w_pos entry) is written; the rest of a capacity-length buffer stays undefined, and the NeRF backwards read
+        # exactly the live rows, so no capacity-sized fill
+        g_w = torch.empty_like(w)
+        gl = contig(g_loss.reshape(1), torch.float32)
+        lib.call('nsr_distortion_bwd', ptr(w), ptr(w_pos), ptr(a), ptr(b), ctx.t_mode, ptr(ray_ids), ptr(gl), ptr(g_w), ray_ids.shape[0],
+                 ptr(n_dev), stream())
+        return g_w, None, None, None, None, None, None
+
+
+def _distortion(w, w_pos, a, b, t_mode, ray_ids, n_dev=None):
+    check_cuda(w, w_pos, a, b, ray_ids, n_dev, what='distortion loss')
+    n = ray_ids.numel()
+    w = contig(w.reshape(-1), torch.float32)
+    a, b = contig(a.reshape(-1), torch.float32), contig(b.reshape(-1), torch.float32)
+    if (w_pos is None and w.numel() < n) or a.numel() < n or b.numel() < n:
+        raise ValueError(f'distortion loss: {n} samples but {w.numel()} weights / {a.numel()} / {b.numel()} per-sample values')
+    return _Distortion.apply(w, None if w_pos is None else contig(w_pos.reshape(-1), torch.int64), a, b, t_mode,
+                             contig(ray_ids.reshape(-1), torch.int32), None if n_dev is None else contig(n_dev.reshape(-1)[:1], torch.int64))
+
+
+def flatten_eff_distloss(w, m, interval, ray_id):
+    """Distortion loss of mip-NeRF 360 over packed samples sorted by ray, with the signature and semantics of
+    ``torch_efficient_distloss.flatten_eff_distloss`` (systems/nerf.py:103-106, systems/neus.py:131-139):
+
+        sum_rays [ sum_ij w_i w_j |m_i - m_j| + 1/3 sum_i w_i^2 interval_i ] / (max(ray_id) + 1)
+
+    w, m [K] (midpoints non-decreasing along each ray), interval [K] or a Python scalar, ray_id int32 / int64 [K] sorted.  The gradient
+    flows to ``w`` only.  One CUDA kernel each way (csrc/distloss.cu), stable prefix recurrences, no host synchronisation.  K = 0 gives a
+    zero loss (the package raises there: ``max()`` of an empty tensor)."""
+    check_cuda(w, m, ray_id, what='flatten_eff_distloss')
+    if not torch.is_tensor(interval):
+        interval = torch.full((ray_id.numel(),), float(interval), device=w.device)
+    elif interval.numel() == 1:
+        interval = interval.reshape(1).expand(ray_id.numel())
+    return _distortion(w, None, m, interval, 0, ray_id)
+
+
+def distortion_loss(out, suffix=''):
+    """Distortion loss of a model's training output dict (``out['weights' + suffix]`` etc.), whatever layout produced it -- the caller
+    does not need to know which.  suffix='_bg': the NeuS learned-background term (systems/neus.py:136-139).
+
+      fused NeRF, static (``loose_pos``): loose-layout weights gathered through loose_pos, packed t_starts / t_ends, live count
+          offsets_packed[n_rays] -- the graphed C2 step;
+      two-pass NeRF, static (``t_starts`` without ``points``): packed buffers, live count num_samples;
+      NeuS, static (``num_samples_dev``): points / intervals, live count num_samples_dev;
+      every exact-size dict: weights / points / intervals / ray_indices.
+    All forms are capturable into a CUDA graph; rows past the live count are neither read nor written."""
+    g = lambda k: out[k + suffix]
+    if 'loose_pos' + suffix in out:
+        return _distortion(g('weights'), g('loose_pos'), g('t_starts'), g('t_ends'), 1, g('ray_indices'), g('offsets_packed')[-1:])
+    if 't_starts' + suffix in out and 'points' + suffix not in out:
+        return _distortion(g('weights'), None, g('t_starts'), g('t_ends'), 1, g('ray_indices'), g('num_samples'))
+    return _distortion(g('weights'), None, g('points'), g('intervals'), 0, g('ray_indices'), out.get('num_samples_dev' + suffix))

@@ -305,13 +305,17 @@ def accumulate_along_rays(weights, ray_indices, values=None, n_rays=None):
 
 
 def install_as_reference_modules():
-    """Make ``import tinycudann`` / ``import nerfacc`` (as written in the reference's models/*.py)
-    resolve to this package, so the reference's model code runs unmodified on our kernels."""
+    """Make ``import tinycudann`` / ``import nerfacc`` (as written in the reference's models/*.py) and
+    ``from torch_efficient_distloss import flatten_eff_distloss`` (systems/nerf.py:4, systems/neus.py:4)
+    resolve to this package, so the reference's model and system code runs unmodified on our kernels."""
     import sys
-    from . import tcnn as _tcnn
+    from . import tcnn as _tcnn, losses as _losses
     this = sys.modules[__name__]
     sys.modules.setdefault('tinycudann', _tcnn)
     sys.modules.setdefault('nerfacc', this)
     inter = types.ModuleType('nerfacc.intersection')
     inter.ray_aabb_intersect = ray_aabb_intersect
     sys.modules.setdefault('nerfacc.intersection', inter)
+    distloss = types.ModuleType('torch_efficient_distloss')
+    distloss.flatten_eff_distloss = _losses.flatten_eff_distloss
+    sys.modules.setdefault('torch_efficient_distloss', distloss)
