@@ -61,35 +61,12 @@ static_assert(kSmemBytes <= 227 * 1024, "shared memory");
 // barrier slots (8 bytes each)
 enum { B_FULL0 = 0, B_FULL1, B_EMPTY0, B_EMPTY1, B_DEFULL0, B_DEFULL1, B_DEEMPTY0, B_DEEMPTY1, B_COUNT };
 
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
 __device__ __forceinline__ void tma_bulk(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
                : "memory");
-}
-// bounded wait: a barrier that is never signalled (a bug) sets *status and traps instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* status, int code) {
-  const long long t0 = clock64();
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}\n"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (clock64() - t0 > 4000000000ll) {
-      if (status) atomicExch(status, code);
-      __trap();
-    }
-  }
 }
 // barrier of the 128 threads of chain warpgroup c (ids 1, 2); id 3 joins both chain warpgroups
 __device__ __forceinline__ void wg_bar(int c) { asm volatile("bar.sync %0, 128;" ::"r"(1 + c) : "memory"); }
@@ -108,9 +85,7 @@ __device__ __forceinline__ void stage_canonical(uint8_t* dst, const __half* __re
 //   K-major  [rows][K]: LBO = 128 B (the two 8-wide K chunks), SBO = (K/8)*128 B (8-row groups); step kk starts 256 B further
 //   MN-major [k rows][C] read with M / N along C: SBO = 128 B (8-column chunks), LBO = (C/8)*128 B (8-row k groups); step kk = 2 LBO
 __device__ __forceinline__ uint64_t dk(uint32_t addr, int K, int kk) { return nsr_wg_desc(addr + 256u * (uint32_t)kk, 128u, (uint32_t)(K / 8) * 128u); }
-__device__ __forceinline__ uint64_t dm(uint32_t addr, int C, int kk) {
-  return nsr_wg_desc(addr + 2u * (uint32_t)(C / 8) * 128u * (uint32_t)kk, (uint32_t)(C / 8) * 128u, 128u);
-}
+__device__ __forceinline__ uint64_t dm(uint32_t addr, int C, int kk) { return nsr_wg_desc_mn(addr, C, kk); }
 
 struct TcArgs {
   const uint8_t* enc_tiles;  // canonical [tile][128][32] fp16

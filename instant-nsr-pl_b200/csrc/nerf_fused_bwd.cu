@@ -7,8 +7,11 @@
 // levels) with 8-byte vector REDs into the fp32 gradient table, then split the five weight-gradient GEMMs
 // (dW = dPre^T * Act, K = 64 samples) over the 4 warps with register accumulators that persist for the whole
 // kernel; one atomicAdd per weight per CTA at the end (tcnn: split-K CUTLASS GEMMs over K = batch + reduction).
+// The split backward's network half (nerf_bwd_net_kernel, below) runs the same chain but hands the weight-gradient GEMMs to a wgmma
+// warpgroup.
 #include <stdlib.h>
 #include "nerf_fused.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
@@ -83,9 +86,8 @@ __device__ __forceinline__ void relu_mask_pack(const float (&acc)[1][8][4], cons
 // every row (written by nsr_pack_kept; buffers padded by one tile).  All global inputs of tile t+1 are then fetched with cp.async
 // into the second smem buffer while tile t computes: no load of the kernel sits in front of the math any more (ncu before:
 // 37 % of the stall samples were long-scoreboard waits on the row_pos -> enc / ray_indices -> rays chains and on the tile's loads).
-// SCATTER = false (split backward, nsr_nerf_field_bwd_split): d(encoding) leaves the kernel as fp16 pairs [n][16 levels] (still multiplied by
-// the loss scale) and a second, high-occupancy kernel (nerf_table_scatter_kernel) turns it into table REDs with warp-wide run merging.
-template <bool PACKED, bool SCATTER>
+// The split backward (d(encoding) to memory, REDs in a separate kernel) uses nerf_bwd_net_kernel below instead.
+template <bool PACKED>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __grid_constant__ nsr_nerf_t P, const float* __restrict__ rays,
                                                                const int32_t* __restrict__ ray_indices, const float* __restrict__ t_starts,
                                                                const float* __restrict__ t_ends, const __half* __restrict__ enc_save,
@@ -93,7 +95,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
                                                                const float* __restrict__ d_sraw, const float* __restrict__ d_rgb,
                                                                float* __restrict__ grad_dparams, float* __restrict__ grad_cparams,
                                                                float loss_scale, const float* __restrict__ amax_ptr, int64_t n_cap, const int64_t* __restrict__ n_dev,
-                                                               const int64_t* __restrict__ row_pos, const float* __restrict__ xyzdir, uint32_t* __restrict__ denc_out) {
+                                                               const int64_t* __restrict__ row_pos, const float* __restrict__ xyzdir) {
   const int64_t n = n_dev ? min(*n_dev, n_cap) : n_cap;
   extern __shared__ __align__(16) __half smem[];
   __half* T = smem + NF_W_TOTAL;
@@ -279,18 +281,8 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
     // Levels 0..7 (nt < 2): consecutive samples of a ray stay in one cell for several steps, so the 8 lanes that hold the
     // same level for 8 consecutive samples first merge runs of equal cells with a segmented shuffle scan and only the
     // last lane of each run issues the 8 REDs (-40 % REDs overall, far less same-address contention in L2).
-    if (!SCATTER) {  // split backward: 4 lanes (c = 0..3) x 4-byte stores = 16 contiguous bytes per (row, nt)
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int64_t i = hh ? ib : ia;
-        if (i < n) {
-#pragma unroll
-          for (int nt = 0; nt < 4; ++nt) denc_out[i * 16 + nt * 4 + c] = nsr_pack_h2(accE[0][nt][hh * 2], accE[0][nt][hh * 2 + 1]);
-        }
-      }
-    }
-#pragma unroll
-    for (int hh = 0; hh < (SCATTER ? 2 : 0); ++hh) {
+    for (int hh = 0; hh < 2; ++hh) {
       const int64_t i = hh ? ib : ia;
       const bool ok = i < n;
       float x = 0.f, y = 0.f, z = 0.f, dx, dy, dz;
@@ -377,6 +369,301 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
         const int o = w.m0 + g + ((i >> 1) << 3), ii = w.n0 + j * 8 + c * 2 + (i & 1);
         atomicAdd(dst + (size_t)o * w.in_dim + ii, wacc[s][j][i] * inv_scale);
       }
+  }
+}
+
+// ==== network half of the split backward (nsr_nerf_field_bwd_net / _split) =====================================================
+// One CTA per SM, 12 warps, persistent over the CTA's 64-row tiles of packed rows (tile = blockIdx.x + it * gridDim.x):
+//   warps 0-3, 4-7   two chain groups that take the CTA's tiles in turn (group = it & 1).  A group runs the same warp-level code as
+//                    nerf_bwd_kernel -- mma.sync forward recompute and dgrad chain in registers, 16 rows per warp, the same fp16 rounding
+//                    points, ReLU masks and loss scale -- writes d(encoding) to global memory, and leaves every activation and
+//                    pre-activation gradient the weight gradients need in a tile slot, in wgmma's canonical no-swizzle layout.
+//                    Each group prefetches its next tile's inputs (cp.async, 7.5 KB) into its own stage while it computes.
+//   warps 8-11       one warpgroup that runs the five weight-gradient GEMMs of every tile (K = the tile's 64 rows) as wgmma.mma_async
+//                    with both operands read from the slot (MN-major descriptors over the K-major tiles: no transposes).  dDW2 and dCW3
+//                    (16 outputs) are computed transposed so that M = 64.  The 80 fp32 accumulators per thread live in registers for the
+//                    whole kernel; one atomicAdd per weight per CTA at the end.
+// Three slots form a ring (tile it -> slot it % 3): mbarrier FULL[s] hands a slot from its chain group to the warpgroup, EMPTY[s] back.
+// Rows past the live count hold zeros in every slot operand: their encodings and per-row inputs are zeroed in the stage, and every
+// layer maps zero inputs to zero.
+constexpr int kNetThreads = 384;
+// one tile slot (bytes), canonical [64][K] fp16 tiles
+constexpr int SL_X0 = 0;                    // [64][32] encoded features
+constexpr int SL_CI = SL_X0 + kRows * 32 * 2;   // [64][32] colour input: out16 | SH16
+constexpr int SL_H1 = SL_CI + kRows * 32 * 2;   // [64][64] density hidden (post ReLU)
+constexpr int SL_G1 = SL_H1 + kRows * 64 * 2;   // [64][64]
+constexpr int SL_G2 = SL_G1 + kRows * 64 * 2;   // [64][64]
+constexpr int SL_DC3 = SL_G2 + kRows * 64 * 2;  // [64][16] d(rgb pre-activation), columns 3..15 zero
+constexpr int SL_DO = SL_DC3 + kRows * 16 * 2;  // [64][16] d(out16)
+constexpr int SL_DG2 = SL_DO + kRows * 16 * 2;  // [64][64]
+constexpr int SL_DG1 = SL_DG2 + kRows * 64 * 2; // [64][64]
+constexpr int SL_DH1 = SL_DG1 + kRows * 64 * 2; // [64][64]
+constexpr int kSlotBytes = SL_DH1 + kRows * 64 * 2;  // 61440
+constexpr int kNetSlots = 3;
+// CTA map (bytes): padded weights | slots | two input stages (encodings [64][40] halves + the per-row floats) | mbarriers
+constexpr int N_SLOTS = NF_W_TOTAL * 2;
+constexpr int N_STAGE = N_SLOTS + kNetSlots * kSlotBytes;
+constexpr int kStageBytes = kRows * NF_LD32 * 2 + S_ROWF * 4;  // 7680
+constexpr int N_BARS = N_STAGE + 2 * kStageBytes;
+constexpr size_t kNetSmemBytes = N_BARS + 2 * kNetSlots * 8;
+static_assert(N_SLOTS % 128 == 0 && kSlotBytes % 128 == 0 && kStageBytes % 16 == 0 && N_BARS % 8 == 0, "alignment");
+static_assert(kNetSmemBytes <= 227 * 1024, "shared memory");
+
+// A fragments <-> canonical [rows][K] tile (the fragment layout of nsr_load_afrag / nsr_store_afrag; 128-byte core matrices keep both
+// conflict-free)
+template <int KT>
+__device__ __forceinline__ void canon_load_afrag(uint32_t (&a)[1][KT][4], const uint8_t* tile, int K, int row0, int col0 = 0) {
+  const int lane = threadIdx.x & 31, mi = lane >> 3, r = lane & 7;
+#pragma unroll
+  for (int k = 0; k < KT; ++k) nsr_ldmatrix_x4(a[0][k], tile + nsr_canon_off(row0 + (mi & 1) * 8 + r, col0 + k * 16 + (mi >> 1) * 8, K));
+}
+template <int KT>
+__device__ __forceinline__ void canon_store_afrag(const uint32_t (&a)[1][KT][4], uint8_t* tile, int K, int row0, int col0 = 0) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
+#pragma unroll
+  for (int k = 0; k < KT; ++k) {
+    const int col = col0 + k * 16 + c * 2;
+    *reinterpret_cast<uint32_t*>(tile + nsr_canon_off(row0 + g, col, K)) = a[0][k][0];
+    *reinterpret_cast<uint32_t*>(tile + nsr_canon_off(row0 + g + 8, col, K)) = a[0][k][1];
+    *reinterpret_cast<uint32_t*>(tile + nsr_canon_off(row0 + g, col + 8, K)) = a[0][k][2];
+    *reinterpret_cast<uint32_t*>(tile + nsr_canon_off(row0 + g + 8, col + 8, K)) = a[0][k][3];
+  }
+}
+__device__ __forceinline__ void group_bar(int grp) { asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory"); }
+
+// flush one weight-gradient accumulator (m64nN layout) into dst[m * stride_m + n * stride_n]
+template <int R>
+__device__ __forceinline__ void net_flush(const float (&w)[R], float* dst, int stride_m, int stride_n, float inv_scale) {
+  const int lane = threadIdx.x & 31, m0 = 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const int j = r >> 2, h = (r >> 1) & 1, e = r & 1;
+    atomicAdd(dst + (size_t)(m0 + 8 * h) * stride_m + (size_t)(8 * j + c0 + e) * stride_n, w[r] * inv_scale);
+  }
+}
+
+__global__ void __launch_bounds__(kNetThreads, 1) nerf_bwd_net_kernel(const __half* __restrict__ enc_save, const __half* __restrict__ dparams,
+                                                                      const __half* __restrict__ cparams, const float* __restrict__ d_sraw,
+                                                                      const float* __restrict__ d_rgb, float* __restrict__ grad_dparams,
+                                                                      float* __restrict__ grad_cparams, float loss_scale,
+                                                                      const float* __restrict__ amax_ptr, int64_t n_cap,
+                                                                      const int64_t* __restrict__ n_dev, const float* __restrict__ xyzdir,
+                                                                      uint32_t* __restrict__ denc_out) {
+  const int64_t n = n_dev ? min(*n_dev, n_cap) : n_cap;
+  extern __shared__ __align__(128) uint8_t smem_net[];
+  __half* W = reinterpret_cast<__half*>(smem_net);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (loss_scale <= 0.f) {  // automatic: the same rule as nerf_bwd_kernel
+    const float amax = fmaxf(__ldg(amax_ptr), 1e-30f);
+    loss_scale = exp2f(fminf(fmaxf(floorf(log2f(256.f / amax)), -24.f), 60.f));
+  }
+  const float inv_scale = 1.f / loss_scale;
+  const uint32_t sbase = nsr_smem_u32(smem_net);
+  auto full_bar = [&](int s) { return sbase + N_BARS + 8u * (uint32_t)s; };
+  auto empty_bar = [&](int s) { return sbase + N_BARS + 8u * (uint32_t)(kNetSlots + s); };
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kNetSlots; ++s) {
+      mbar_init(full_bar(s), 128);   // the 128 threads of the chain group that filled the slot
+      mbar_init(empty_bar(s), 128);  // the 128 threads of the weight-gradient warpgroup
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  nf_stage_weights(W, dparams, cparams, true);
+  __syncthreads();
+  const int64_t n_tiles = (n + kRows - 1) / kRows;
+  const int64_t my_tiles = n_tiles > (int64_t)blockIdx.x ? (n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+
+  if (warp < 8) {
+    // ================================ chain groups ================================
+    const int grp = warp >> 2, gtid = threadIdx.x & 127, g = lane >> 2, c = lane & 3;
+    const int r0 = (warp & 3) * 16;
+    __half* sx = reinterpret_cast<__half*>(smem_net + N_STAGE + grp * kStageBytes);  // [64][40] encodings of the group's next tile
+    float* rf = reinterpret_cast<float*>(smem_net + N_STAGE + grp * kStageBytes + kRows * NF_LD32 * 2);
+    auto fetch_tile = [&](int64_t it) {  // inputs of the CTA's tile `it` -> this group's stage (16-byte chunks, L1 bypassed)
+      const int64_t row0 = ((int64_t)blockIdx.x + it * gridDim.x) * kRows;
+      for (int v = gtid; v < kRows * 4; v += 128) cp_async16(sx + (v >> 2) * NF_LD32 + (v & 3) * 8, enc_save + (row0 + (v >> 2)) * 32 + (v & 3) * 8);
+      if (gtid < kRows * 6 / 4) cp_async16(rf + S_XYZ + gtid * 4, xyzdir + row0 * 6 + gtid * 4);
+      if (gtid < kRows / 4) cp_async16(rf + S_DS + gtid * 4, d_sraw + row0 + gtid * 4);
+      if (gtid >= 64 && gtid < 64 + kRows * 3 / 4) cp_async16(rf + S_DRGB + (gtid - 64) * 4, d_rgb + row0 * 3 + (gtid - 64) * 4);
+      cp_async_commit();
+    };
+    if (grp < my_tiles) fetch_tile(grp);
+    for (int64_t it = grp; it < my_tiles; it += 2) {
+      const int s = (int)(it % kNetSlots);
+      const int64_t row0 = ((int64_t)blockIdx.x + it * gridDim.x) * kRows;
+      cp_async_wait_all();
+      group_bar(grp);  // the group's copies have all landed
+      if (row0 + kRows > n) {  // last, partial tile: rows >= n hold stale data; zero them so that 0 * garbage never reaches the wgrad sums
+        for (int v = gtid; v < kRows * 4; v += 128)
+          if (row0 + (v >> 2) >= n) *reinterpret_cast<uint4*>(sx + (v >> 2) * NF_LD32 + (v & 3) * 8) = make_uint4(0, 0, 0, 0);
+        for (int v = gtid; v < S_ROWF; v += 128) {
+          const int r = v < S_DS ? v / 6 : (v < S_DRGB ? v - S_DS : (v - S_DRGB) / 3);
+          if (row0 + r >= n) rf[v] = 0.f;
+        }
+        group_bar(grp);
+      }
+      if (it >= kNetSlots) mbar_wait(empty_bar(s), (uint32_t)((it / kNetSlots - 1) & 1), nullptr, 0);  // tile it - 3's wgrad is done
+      uint8_t* slot = smem_net + N_SLOTS + s * kSlotBytes;
+      const int64_t ia = row0 + r0 + g, ib = ia + 8;
+      // ---- this warp's 16 rows: encoded features (-> slot X0) and SH of the view direction (-> CI columns 16..31); per-row gradients
+      uint32_t a_in[1][2][4];
+      nsr_load_afrag<1, 2>(a_in, sx, NF_LD32, r0);
+      canon_store_afrag<2>(a_in, slot + SL_X0, 32, r0);
+      if (lane < 16) {
+        uint4 s0 = make_uint4(0, 0, 0, 0), s1 = s0;
+        if (row0 + r0 + lane < n) {
+          float sh[16];
+          const float* rr = rf + S_XYZ + (r0 + lane) * 6;
+          nsr_sh4(rr[3], rr[4], rr[5], sh);
+          s0 = make_uint4(nsr_pack_h2(sh[0], sh[1]), nsr_pack_h2(sh[2], sh[3]), nsr_pack_h2(sh[4], sh[5]), nsr_pack_h2(sh[6], sh[7]));
+          s1 = make_uint4(nsr_pack_h2(sh[8], sh[9]), nsr_pack_h2(sh[10], sh[11]), nsr_pack_h2(sh[12], sh[13]), nsr_pack_h2(sh[14], sh[15]));
+        }
+        *reinterpret_cast<uint4*>(slot + SL_CI + nsr_canon_off(r0 + lane, 16, 32)) = s0;
+        *reinterpret_cast<uint4*>(slot + SL_CI + nsr_canon_off(r0 + lane, 24, 32)) = s1;
+      }
+      float drgb[2][2], dsr[2];  // (row g / g+8) x (columns 2c, 2c+1 < 3); d sigma_raw of rows g, g+8
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) drgb[hh][e] = (c * 2 + e < 3) ? rf[S_DRGB + (r0 + g + hh * 8) * 3 + c * 2 + e] : 0.f;
+        dsr[hh] = rf[S_DS + r0 + g + hh * 8];
+      }
+      group_bar(grp);  // the whole group is done with the stage: refill it with the group's next tile
+      if (it + 2 < my_tiles) fetch_tile(it + 2);
+
+      // ---- forward recompute
+      uint32_t a_h1[1][4][4], a_o[1][1][4], a_g1[1][4][4], a_g2[1][4][4];
+      float acc[1][8][4], acc16[1][2][4];
+      nsr_zero_acc(acc);
+      nsr_gemm_w<1, 2, 8>(acc, a_in, W + NF_OFF_DW1, NF_LD32);
+      nsr_acc_to_afrag<1, 8>(acc, a_h1, NSR_ACT_RELU);
+      canon_store_afrag<4>(a_h1, slot + SL_H1, 64, r0);
+      nsr_zero_acc(acc16);
+      nsr_gemm_w<1, 4, 2>(acc16, a_h1, W + NF_OFF_DW2, NSR_LD64);
+      nsr_acc_to_afrag<1, 2>(acc16, a_o, NSR_ACT_NONE);
+      canon_store_afrag<1>(a_o, slot + SL_CI, 32, r0);
+      __syncwarp();
+      {
+        uint32_t a_c[1][2][4], a_sh[1][1][4];
+        canon_load_afrag<1>(a_sh, slot + SL_CI, 32, r0, 16);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          a_c[0][0][j] = a_o[0][0][j];
+          a_c[0][1][j] = a_sh[0][0][j];
+        }
+        nsr_zero_acc(acc);
+        nsr_gemm_w<1, 2, 8>(acc, a_c, W + NF_OFF_CW1, NF_LD32);
+      }
+      nsr_acc_to_afrag<1, 8>(acc, a_g1, NSR_ACT_RELU);
+      canon_store_afrag<4>(a_g1, slot + SL_G1, 64, r0);
+      nsr_zero_acc(acc);
+      nsr_gemm_w<1, 4, 8>(acc, a_g1, W + NF_OFF_CW2, NSR_LD64);
+      nsr_acc_to_afrag<1, 8>(acc, a_g2, NSR_ACT_RELU);
+      canon_store_afrag<4>(a_g2, slot + SL_G2, 64, r0);
+      nsr_zero_acc(acc16);
+      nsr_gemm_w<1, 4, 2>(acc16, a_g2, W + NF_OFF_CW3, NSR_LD64);
+      // ---- d(rgb pre-activation) = d_rgb * s (1 - s), s = sigmoid(fp16(raw)); columns 0..2 only
+      uint32_t a_dc3[1][1][4];
+      {
+        float dp[4] = {0.f, 0.f, 0.f, 0.f};  // (row g: col c*2, c*2+1), (row g+8: col c*2, c*2+1)
+        if (c < 2) {
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            if ((hh ? ib : ia) < n) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                if (c * 2 + e < 3) {
+                  const float raw = __half2float(__float2half_rn(acc16[0][0][hh * 2 + e]));
+                  const float sg = 1.f / (1.f + expf(-raw));
+                  dp[hh * 2 + e] = drgb[hh][e] * sg * (1.f - sg) * loss_scale;
+                }
+              }
+            }
+          }
+        }
+        a_dc3[0][0][0] = nsr_pack_h2(dp[0], dp[1]);
+        a_dc3[0][0][1] = nsr_pack_h2(dp[2], dp[3]);
+        a_dc3[0][0][2] = 0u;
+        a_dc3[0][0][3] = 0u;
+        canon_store_afrag<1>(a_dc3, slot + SL_DC3, 16, r0);
+      }
+      // ---- dgrad chain
+      uint32_t a_d[1][4][4];
+      nsr_zero_acc(acc);
+      nsr_gemm_wt<1, 1, 8>(acc, a_dc3, W + NF_OFF_CW3, NSR_LD64);
+      relu_mask_pack(acc, a_g2, a_d);
+      canon_store_afrag<4>(a_d, slot + SL_DG2, 64, r0);
+      nsr_zero_acc(acc);
+      nsr_gemm_wt<1, 4, 8>(acc, a_d, W + NF_OFF_CW2, NSR_LD64);
+      relu_mask_pack(acc, a_g1, a_d);
+      canon_store_afrag<4>(a_d, slot + SL_DG1, 64, r0);
+      nsr_zero_acc(acc16);
+      nsr_gemm_wt<1, 4, 2>(acc16, a_d, W + NF_OFF_CW1, NF_LD32);  // first 16 input columns = the geometry features
+      if (c == 0) {  // density path: d(out0) += d sigma / d raw (trunc_exp backward folded in by nsr_nerf_ray_bwd)
+        if (ia < n) acc16[0][0][0] += dsr[0] * loss_scale;
+        if (ib < n) acc16[0][0][2] += dsr[1] * loss_scale;
+      }
+      uint32_t a_do[1][1][4];
+      nsr_acc_to_afrag<1, 2>(acc16, a_do, NSR_ACT_NONE);
+      canon_store_afrag<1>(a_do, slot + SL_DO, 16, r0);
+      nsr_zero_acc(acc);
+      nsr_gemm_wt<1, 1, 8>(acc, a_do, W + NF_OFF_DW2, NSR_LD64);
+      relu_mask_pack(acc, a_h1, a_d);
+      canon_store_afrag<4>(a_d, slot + SL_DH1, 64, r0);
+      // the slot is complete: make this thread's stores visible to the tensor core and hand the slot over
+      nsr_proxy_fence();
+      mbar_arrive(full_bar(s));
+      float accE[1][4][4];
+      nsr_zero_acc(accE);
+      nsr_gemm_wt<1, 4, 4>(accE, a_d, W + NF_OFF_DW1, NF_LD32);
+      // ---- d(encoding) -> fp16 pairs [n][16 levels], still multiplied by the loss scale: 4 lanes x 4 bytes = 16 contiguous bytes per (row, nt)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int64_t i = hh ? ib : ia;
+        if (i < n) {
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt) denc_out[i * 16 + nt * 4 + c] = nsr_pack_h2(accE[0][nt][hh * 2], accE[0][nt][hh * 2 + 1]);
+        }
+      }
+    }
+  } else {
+    // ================================ weight-gradient warpgroup ================================
+    float w_dw1[16], w_dw2t[8], w_cw1[16], w_cw2[32], w_cw3t[8];  // m64 x n32 / n16 / n32 / n64 / n16
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      if (i < 8) w_dw2t[i] = w_cw3t[i] = 0.f;
+      if (i < 16) w_dw1[i] = w_cw1[i] = 0.f;
+      w_cw2[i] = 0.f;
+    }
+    for (int64_t it = 0; it < my_tiles; ++it) {
+      const int s = (int)(it % kNetSlots);
+      mbar_wait(full_bar(s), (uint32_t)((it / kNetSlots) & 1), nullptr, 0);
+      const uint32_t sl = sbase + N_SLOTS + (uint32_t)s * kSlotBytes;
+      nsr_wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {  // K = 64 rows in four k16 steps
+        nsr_wgmma_n32<1, 1>(w_dw1, nsr_wg_desc_mn(sl + SL_DH1, 64, kk), nsr_wg_desc_mn(sl + SL_X0, 32, kk), 1u);   // dDW1   += dH1^T . X0
+        nsr_wgmma_n16<1, 1>(w_dw2t, nsr_wg_desc_mn(sl + SL_H1, 64, kk), nsr_wg_desc_mn(sl + SL_DO, 16, kk), 1u);   // dDW2^T += H1^T . dO
+        nsr_wgmma_n32<1, 1>(w_cw1, nsr_wg_desc_mn(sl + SL_DG1, 64, kk), nsr_wg_desc_mn(sl + SL_CI, 32, kk), 1u);   // dCW1   += dG1^T . CI
+        nsr_wgmma_n64<1, 1>(w_cw2, nsr_wg_desc_mn(sl + SL_DG2, 64, kk), nsr_wg_desc_mn(sl + SL_G1, 64, kk), 1u);   // dCW2   += dG2^T . G1
+        nsr_wgmma_n16<1, 1>(w_cw3t, nsr_wg_desc_mn(sl + SL_G2, 64, kk), nsr_wg_desc_mn(sl + SL_DC3, 16, kk), 1u);  // dCW3^T += G2^T . dC3
+      }
+      nsr_wg_commit();
+      nsr_wg_wait0();
+      nsr_wg_fence_regs(w_dw1);
+      nsr_wg_fence_regs(w_dw2t);
+      nsr_wg_fence_regs(w_cw1);
+      nsr_wg_fence_regs(w_cw2);
+      nsr_wg_fence_regs(w_cw3t);
+      mbar_arrive(empty_bar(s));
+    }
+    if (my_tiles > 0) {
+      net_flush(w_dw1, grad_dparams, 32, 1, inv_scale);                           // dDW1 [out m][in n]
+      net_flush(w_dw2t, grad_dparams + 64 * 32, 1, 64, inv_scale);                // dDW2^T [in m][out n] -> DW2 [out][in]
+      net_flush(w_cw1, grad_cparams, 32, 1, inv_scale);                           // dCW1 [out m][in n]
+      net_flush(w_cw2, grad_cparams + 64 * 32, 64, 1, inv_scale);                 // dCW2 [out m][in n]
+      net_flush(w_cw3t, grad_cparams + 64 * 32 + 64 * 64, 1, 64, inv_scale);      // dCW3^T [in m][out n] -> CW3 [out][in]
+    }
   }
 }
 
@@ -473,19 +760,17 @@ __global__ void __launch_bounds__(256, MINB) nerf_table_scatter_kernel(const __g
 int field_bwd_launch(const nsr_nerf_t* f, const float* rays, const int32_t* ray_indices, const float* t_starts, const float* t_ends,
                      const void* enc_save_h, const void* dparams_h, const void* cparams_h, const float* d_sraw, const float* d_rgb,
                      float* grad_dparams, float* grad_cparams, float loss_scale, const float* amax, int64_t k, const int64_t* k_dev,
-                     const int64_t* row_pos, const float* xyzdir, void* denc_out, void* stream, const char* who) {
+                     const int64_t* row_pos, const float* xyzdir, void* stream, const char* who) {
   NSR_REQUIRE(f != nullptr, "%s: field descriptor is NULL", who);
   NSR_REQUIRE(f->grid.n_levels == 16 && f->grid.n_features == 2 && f->feature_dim == 16 && f->density_hidden == 1 && f->color_hidden == 2,
               "%s: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2", who);
   NSR_REQUIRE(loss_scale > 0.f || amax != nullptr, "%s: loss_scale <= 0 (automatic) needs the amax pointer", who);
   if (k == 0) return 0;
   NSR_REQUIRE(xyzdir == nullptr || row_pos == nullptr, "%s: packed inputs (xyzdir) and row_pos are mutually exclusive", who);
-  NSR_REQUIRE(denc_out == nullptr || xyzdir != nullptr, "%s: the split form needs the packed inputs (xyzdir)", who);
   static thread_local bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(nerf_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(nerf_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(nerf_bwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(nerf_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(nerf_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e != cudaSuccess) {
       nsr_set_error("%s: cannot reserve %zu B shared memory: %s", who, kSmemBytes, cudaGetErrorString(e));
       return 2;
@@ -497,14 +782,40 @@ int field_bwd_launch(const nsr_nerf_t* f, const float* rays, const int32_t* ray_
   if (k_dev != nullptr) grid = nsr_sm_count() * kCtasPerSm;
 #define NSR_BWD_ARGS                                                                                                                        \
   *f, rays, ray_indices, t_starts, t_ends, (const __half*)enc_save_h, (const __half*)dparams_h, (const __half*)cparams_h, d_sraw, d_rgb,    \
-      grad_dparams, grad_cparams, loss_scale, amax, k, k_dev, row_pos, xyzdir, (uint32_t*)denc_out
-  if (denc_out != nullptr)
-    nerf_bwd_kernel<true, false><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
-  else if (xyzdir != nullptr)
-    nerf_bwd_kernel<true, true><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
+      grad_dparams, grad_cparams, loss_scale, amax, k, k_dev, row_pos, xyzdir
+  if (xyzdir != nullptr)
+    nerf_bwd_kernel<true><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
   else
-    nerf_bwd_kernel<false, true><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
+    nerf_bwd_kernel<false><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
 #undef NSR_BWD_ARGS
+  NSR_CHECK_LAUNCH(who);
+  return 0;
+}
+
+// network half of the split backward: nerf_bwd_net_kernel, one CTA per SM
+int field_bwd_net_launch(const nsr_nerf_t* f, const void* enc_k_h, const void* dparams_h, const void* cparams_h, const float* d_sraw,
+                         const float* d_rgb, float* grad_dparams, float* grad_cparams, float loss_scale, const float* amax, int64_t k,
+                         const int64_t* k_dev, const float* xyzdir, void* denc_h, void* stream, const char* who) {
+  NSR_REQUIRE(f != nullptr, "%s: field descriptor is NULL", who);
+  NSR_REQUIRE(f->grid.n_levels == 16 && f->grid.n_features == 2 && f->feature_dim == 16 && f->density_hidden == 1 && f->color_hidden == 2,
+              "%s: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2", who);
+  NSR_REQUIRE(loss_scale > 0.f || amax != nullptr, "%s: loss_scale <= 0 (automatic) needs the amax pointer", who);
+  NSR_REQUIRE(denc_h != nullptr && xyzdir != nullptr, "%s: denc / xyzdir is NULL", who);
+  if (k == 0) return 0;
+  static thread_local bool attr_set = false;
+  if (!attr_set) {
+    const cudaError_t e = cudaFuncSetAttribute(nerf_bwd_net_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kNetSmemBytes);
+    if (e != cudaSuccess) {
+      nsr_set_error("%s: cannot reserve %zu B shared memory: %s", who, kNetSmemBytes, cudaGetErrorString(e));
+      return 2;
+    }
+    attr_set = true;
+  }
+  const int64_t tiles = (k + kRows - 1) / kRows;
+  const int grid = k_dev != nullptr ? nsr_sm_count() : (int)min((int64_t)nsr_sm_count(), tiles);
+  nerf_bwd_net_kernel<<<grid, kNetThreads, kNetSmemBytes, (cudaStream_t)stream>>>((const __half*)enc_k_h, (const __half*)dparams_h, (const __half*)cparams_h,
+                                                                                  d_sraw, d_rgb, grad_dparams, grad_cparams, loss_scale, amax, k, k_dev,
+                                                                                  xyzdir, (uint32_t*)denc_h);
   NSR_CHECK_LAUNCH(who);
   return 0;
 }
@@ -517,7 +828,7 @@ extern "C" int nsr_nerf_field_bwd(const nsr_nerf_t* f, const float* rays, const 
                                   const float* amax, int64_t k, const int64_t* k_dev, const int64_t* row_pos, const float* xyzdir,
                                   void* stream) {
   return field_bwd_launch(f, rays, ray_indices, t_starts, t_ends, enc_save_h, dparams_h, cparams_h, d_sraw, d_rgb, grad_dparams, grad_cparams,
-                          loss_scale, amax, k, k_dev, row_pos, xyzdir, nullptr, stream, "nsr_nerf_field_bwd");
+                          loss_scale, amax, k, k_dev, row_pos, xyzdir, stream, "nsr_nerf_field_bwd");
 }
 
 // The two halves of the split backward as separate entry points (what the Python side calls, so that each half shows up with its own
@@ -529,9 +840,8 @@ extern "C" int nsr_nerf_field_bwd(const nsr_nerf_t* f, const float* rays, const 
 extern "C" int nsr_nerf_field_bwd_net(const nsr_nerf_t* f, const void* enc_k_h, const void* dparams_h, const void* cparams_h, const float* d_sraw,
                                       const float* d_rgb, float* grad_dparams, float* grad_cparams, float loss_scale, const float* amax, int64_t k,
                                       const int64_t* k_dev, const float* xyzdir, void* denc_h, void* stream) {
-  NSR_REQUIRE(denc_h != nullptr && xyzdir != nullptr, "nsr_nerf_field_bwd_net: denc / xyzdir is NULL");
-  return field_bwd_launch(f, nullptr, nullptr, nullptr, nullptr, enc_k_h, dparams_h, cparams_h, d_sraw, d_rgb, grad_dparams, grad_cparams, loss_scale,
-                          amax, k, k_dev, nullptr, xyzdir, denc_h, stream, "nsr_nerf_field_bwd_net");
+  return field_bwd_net_launch(f, enc_k_h, dparams_h, cparams_h, d_sraw, d_rgb, grad_dparams, grad_cparams, loss_scale, amax, k, k_dev, xyzdir, denc_h,
+                              stream, "nsr_nerf_field_bwd_net");
 }
 
 extern "C" int nsr_nerf_table_scatter(const nsr_grid_t* g, const float* xyz, int32_t stride, const void* denc_h, float loss_scale, const float* amax,
@@ -569,10 +879,9 @@ extern "C" int nsr_nerf_table_scatter(const nsr_grid_t* g, const float* xyz, int
 extern "C" int nsr_nerf_field_bwd_split(const nsr_nerf_t* f, const void* enc_k_h, const void* dparams_h, const void* cparams_h,
                                         const float* d_sraw, const float* d_rgb, float* grad_dparams, float* grad_cparams, float loss_scale,
                                         const float* amax, int64_t k, const int64_t* k_dev, const float* xyzdir, void* denc_h, void* stream) {
-  NSR_REQUIRE(denc_h != nullptr && xyzdir != nullptr, "nsr_nerf_field_bwd_split: denc / xyzdir is NULL");
   NSR_REQUIRE((uintptr_t)denc_h % 8 == 0, "nsr_nerf_field_bwd_split: denc must be 8-byte aligned");
-  const int rc = field_bwd_launch(f, nullptr, nullptr, nullptr, nullptr, enc_k_h, dparams_h, cparams_h, d_sraw, d_rgb, grad_dparams, grad_cparams,
-                                  loss_scale, amax, k, k_dev, nullptr, xyzdir, denc_h, stream, "nsr_nerf_field_bwd_split");
+  const int rc = field_bwd_net_launch(f, enc_k_h, dparams_h, cparams_h, d_sraw, d_rgb, grad_dparams, grad_cparams, loss_scale, amax, k, k_dev, xyzdir,
+                                      denc_h, stream, "nsr_nerf_field_bwd_split");
   if (rc != 0 || k == 0) return rc;
   const int grid = (int)min((int64_t)nsr_sm_count() * 8, (k + 255) / 256);
   nerf_table_scatter_kernel<5><<<k_dev ? nsr_sm_count() * 8 : grid, 256, 0, (cudaStream_t)stream>>>(f->grid, xyzdir, 6, (const __half2*)denc_h, loss_scale, amax,

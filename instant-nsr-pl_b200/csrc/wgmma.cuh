@@ -1,4 +1,4 @@
-// Hopper warpgroup MMA (wgmma.mma_async, sm_90a) helpers shared by the tensor-core kernels (mlp_tc.cu, nerf_bwd_tc.cu).
+// Hopper warpgroup MMA (wgmma.mma_async, sm_90a) helpers shared by the tensor-core kernels (mlp_tc.cu, nerf_bwd_tc.cu, nerf_fused_bwd.cu).
 //
 // Operands live in shared memory in the canonical no-swizzle layout: 8 x 16-byte core matrices.
 //   K-major  [rows][K] tile (K contiguous): LBO = byte distance between the two 8-wide K chunks of one k16 step, SBO = distance between
@@ -20,11 +20,42 @@ __device__ __forceinline__ uint64_t nsr_wg_desc(uint32_t saddr, uint32_t lbo_byt
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
 }
 
+// MN-major descriptor of a canonical [k rows][C] tile read with M / N along C, k16 step kk: SBO = 128 B (8-column chunks), LBO = (C/8)*128 B
+// (8-row k groups); step kk starts 2 LBO further
+__device__ __forceinline__ uint64_t nsr_wg_desc_mn(uint32_t addr, int C, int kk) {
+  return nsr_wg_desc(addr + 2u * (uint32_t)(C / 8) * 128u * (uint32_t)kk, (uint32_t)(C / 8) * 128u, 128u);
+}
+
 __device__ __forceinline__ void nsr_wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void nsr_wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void nsr_wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 // generic-proxy shared-memory writes -> visible to the tensor core (async proxy); followed by a barrier
 __device__ __forceinline__ void nsr_proxy_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// shared-memory mbarriers (addresses from nsr_smem_u32)
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory"); }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+// bounded wait: a barrier that is never signalled (a bug) sets *status (if given) and traps instead of hanging the GPU
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* status, int code) {
+  const long long t0 = clock64();
+  for (;;) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t"
+        "}\n"
+        : "=r"(ok)
+        : "r"(bar), "r"(parity)
+        : "memory");
+    if (ok) return;
+    if (clock64() - t0 > 4000000000ll) {
+      if (status) atomicExch(status, code);
+      __trap();
+    }
+  }
+}
 
 // after nsr_wg_wait0: no read of the accumulator registers may be scheduled in front of the wait
 template <int R>
