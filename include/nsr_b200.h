@@ -325,6 +325,21 @@ int nsr_neus_field_bwd(const nsr_grid_t* g, const float* points, const void* tab
                        const float* b2, float radius, int32_t n_out, const float* g_out, const float* g_sdf, const float* g_grad,
                        const float* amax, float* grad_table, float* dW1, float* db1, float* dW2, float* db2, int64_t n, const int64_t* n_dev,
                        void* stream);
+/* ---- fused NeuS SDF field with finite-difference normals + Laplacian (grad_type 'finite_difference': models/geometry.py:181-199) ----
+ * Same field and weights as nsr_neus_field_*, evaluated at the centre x_0 = (p + r) / 2r and at the six stencil points
+ * (clamp(p +- eps e_a, -r, r) + r) / 2r (true fp32 division); hash levels >= n_active contribute 0 (ProgressiveBandHashGrid mask).
+ * fd_state: device float[3] = {eps, fp32(eps^2), n_active} (read on the device, so a captured graph follows the schedule).
+ * fwd: sdf [n], feature [n,n_out] at the centre; grad [n,3] = 0.5 (s_a+ - s_a-) / eps and laplace [n] = sum_a (s_a+ + s_a- - 2 sdf) / eps^2.
+ *      grad and laplace may both be NULL: centre-only forward.
+ * bwd: upstream g_out [n,n_out], g_sdf [n], g_grad [n,3], g_lap [n] (each may be NULL) -> grad_table f32 (+=), dW1, db1, dW2, db2 (+=);
+ *      the points get no gradient.  Rows >= *n_dev (when n_dev is non-NULL) are neither read nor written. */
+int nsr_neus_field_fd_fwd(const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1, const float* W2,
+                          const float* b2, float radius, int32_t n_out, const float* fd_state, float* sdf, float* grad, float* feature,
+                          float* laplace, int64_t n, const int64_t* n_dev, void* stream);
+int nsr_neus_field_fd_bwd(const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1, const float* W2,
+                          const float* b2, float radius, int32_t n_out, const float* fd_state, const float* g_out, const float* g_sdf,
+                          const float* g_grad, const float* g_lap, float* grad_table, float* dW1, float* db1, float* dW2, float* db2, int64_t n,
+                          const int64_t* n_dev, void* stream);
 /* out[0] = max(|a|, |b|, |c|) over up to three fp32 arrays (NULL / 0 skipped): the bound nsr_neus_field_bwd's amax wants. */
 int nsr_absmax3(const float* a, int64_t na, const float* b, int64_t nb, const float* c, int64_t nc, float* out, int64_t rows_cap,
                 const int64_t* rows_dev /* non-NULL: arrays are [rows_cap, w] with *rows_dev live rows */, void* stream);

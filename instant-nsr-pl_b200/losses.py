@@ -155,3 +155,16 @@ def distortion_loss(out, suffix=''):
     if 't_starts' + suffix in out and 'points' + suffix not in out:
         return _distortion(g('weights'), None, g('t_starts'), g('t_ends'), 1, g('ray_indices'), g('num_samples'))
     return _distortion(g('weights'), None, g('points'), g('intervals'), 0, g('ray_indices'), out.get('num_samples_dev' + suffix))
+
+
+def curvature_loss(out):
+    """The curvature term of systems/neus.py:123-127, ``out['sdf_laplace_samples'].abs().mean()``, without a host sync.  With the
+    static layout (``out['num_samples_dev']``: the model ran in static-shape mode) the mean runs over the live rows only, and the rows
+    past them -- which may hold anything, NaN included -- are masked out, so the term can be captured into a CUDA graph."""
+    lap = out['sdf_laplace_samples'].reshape(-1)
+    k = out.get('num_samples_dev')
+    if k is None:
+        return lap.abs().mean()
+    k = k.reshape(-1)[:1]
+    live = torch.arange(lap.shape[0], device=lap.device) < k
+    return torch.where(live, lap.abs(), torch.zeros((), device=lap.device, dtype=lap.dtype)).sum() / k.clamp_min(1).to(lap.dtype).reshape(())

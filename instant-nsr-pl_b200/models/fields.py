@@ -94,6 +94,13 @@ class VolumeSDF(BaseImplicitGeometry):
         self.finite_difference_eps = self.config.get('finite_difference_eps', 1e-3)
         self._finite_difference_eps = None  # value in use; updated per step when "progressive"
         self._fused = self.config.get('fused', True) and self._fusable()
+        self._fused_fd = self.config.get('fused', True) and self._fusable_fd()
+        # {eps, eps^2, n_active} on the device for the finite-difference kernels; update_step refreshes it in place, so a captured
+        # CUDA graph follows the schedule
+        # (a ProgressiveBandHashGrid masks every level until its first update_step)
+        from .networks import ProgressiveBandHashGrid
+        n_active = 0.0 if isinstance(self.encoding.encoding, ProgressiveBandHashGrid) else 16.0
+        self.register_buffer('_fd_state', torch.tensor([float('nan'), float('nan'), n_active]), persistent=False)
 
     def _fusable(self):
         """the neus-blender / neus-dtu geometry shape (configs/neus-blender.yaml:36-63): include_xyz HashGrid(L=16, F=2) + VanillaMLP
@@ -109,6 +116,34 @@ class VolumeSDF(BaseImplicitGeometry):
                     and 'sdf_activation' not in self.config and 'feature_activation' not in self.config)
         except AttributeError:
             return False
+
+    def _fd_grid(self):
+        """the tcnn.Encoding under the include_xyz wrapper (inside a ProgressiveBandHashGrid for the Neuralangelo config)"""
+        from .networks import ProgressiveBandHashGrid
+        inner = self.encoding.encoding
+        return inner.encoding if isinstance(inner, ProgressiveBandHashGrid) else inner
+
+    def _fusable_fd(self):
+        """the Neuralangelo geometry shape (configs/neuralangelo-dtu-wmask.yaml:18-75): include_xyz HashGrid or ProgressiveBandHashGrid
+        (L=16, F=2) + the same VanillaMLP as _fusable() with finite-difference normals => one forward and one backward kernel for the
+        centre and its six stencil points (csrc/neus_field_fd.cu)"""
+        from .. import tcnn
+        from .networks import VanillaMLP
+        net = self.network
+        try:
+            enc = self._fd_grid()
+            return (self.grad_type == 'finite_difference' and self.encoding.include_xyz and isinstance(enc, tcnn.Encoding)
+                    and enc.grid is not None and enc.grid.n_levels == 16 and enc.grid.n_features == 2
+                    and isinstance(net, VanillaMLP) and net.n_hidden_layers == 1 and net.n_neurons == 64 and net.sphere_init
+                    and self.config.mlp_network_config.get('output_activation', 'none') in (None, 'none') and self.n_output_dims <= 16
+                    and 'sdf_activation' not in self.config and 'feature_activation' not in self.config)
+        except AttributeError:
+            return False
+
+    def _n_active_levels(self):
+        from .networks import ProgressiveBandHashGrid
+        inner = self.encoding.encoding
+        return int(inner.current_level) if isinstance(inner, ProgressiveBandHashGrid) else 16
 
     def _effective_weights(self):
         ws = []
@@ -136,6 +171,27 @@ class VolumeSDF(BaseImplicitGeometry):
         rv = [v if self.training else v.detach() for v in rv]
         return rv[0] if len(rv) == 1 else rv
 
+    def _forward_fused_fd(self, points, with_grad, with_feature, with_laplace):
+        from .. import ops
+        stencil = with_grad or with_laplace
+        if stencil and self._finite_difference_eps is None:
+            raise RuntimeError('VolumeSDF: finite-difference step not set -- call update_step() before the first forward')
+        enc = self._fd_grid()
+        shape = points.shape[:-1]
+        W1, b1, W2, b2 = self._effective_weights()
+        with torch.set_grad_enabled(self.training and torch.is_grad_enabled()):
+            sdf, grad, feat, lap = ops.neus_sdf_fd(enc.grid, self.radius, points.reshape(-1, 3), enc.params, enc._params_half(), W1, b1, W2, b2,
+                                                   self._fd_state, with_grad=stencil)
+        rv = [sdf.reshape(shape)]
+        if with_grad:
+            rv.append(grad.reshape(*shape, 3))
+        if with_feature:
+            rv.append(feat.reshape(*shape, self.n_output_dims))
+        if with_laplace:
+            rv.append(lap.reshape(shape))
+        rv = [v if self.training else v.detach() for v in rv]
+        return rv[0] if len(rv) == 1 else rv
+
     def _query(self, unit_points):
         return self.network(self.encoding(unit_points.reshape(-1, 3)))
 
@@ -148,6 +204,8 @@ class VolumeSDF(BaseImplicitGeometry):
         from ..nerfacc import ContractionType as _CT
         if self._fused and not with_laplace and points.is_cuda and self.contraction_type == _CT.AABB:
             return self._forward_fused(points, with_grad, with_feature)
+        if self._fused_fd and points.is_cuda and self.contraction_type == _CT.AABB:
+            return self._forward_fused_fd(points, with_grad, with_feature, with_laplace)
         analytic = with_grad and self.grad_type == 'analytic'
         with torch.inference_mode(torch.is_inference_mode_enabled() and not analytic):
             with torch.set_grad_enabled(self.training or analytic):
@@ -206,6 +264,11 @@ class VolumeSDF(BaseImplicitGeometry):
             self._finite_difference_eps = 2 * self.config.radius / (hg.base_resolution * hg.per_level_scale ** (level - 1))
         else:
             raise ValueError(f'Unknown finite_difference_eps={self.finite_difference_eps}')
+        eps = self._finite_difference_eps
+        st = self._fd_state   # in place (fill_ kernels, no host sync): a captured graph reads the new schedule on its next replay
+        st[0:1].fill_(eps)
+        st[1:2].fill_(eps ** 2)
+        st[2:3].fill_(float(self._n_active_levels()))
 
 
 @register('volume-radiance')

@@ -183,8 +183,10 @@ class NeuSModel(BaseModel):
 
     def _forward_static(self, rays, jitter=None):
         cfg = self.config
-        if cfg.learned_background or not cfg.grid_prune or cfg.geometry.grad_type != 'analytic' or not rays.is_cuda:
-            raise NotImplementedError("static NeuS forward: foreground-only configs with grid_prune and analytic normals on CUDA (neus-blender)")
+        fd = cfg.geometry.grad_type == 'finite_difference' and getattr(self.geometry, '_fused_fd', False)
+        if cfg.learned_background or not cfg.grid_prune or not (cfg.geometry.grad_type == 'analytic' or fd) or not rays.is_cuda:
+            raise NotImplementedError("static NeuS forward: foreground-only configs with grid_prune and analytic normals (neus-blender) or "
+                                      "fused finite-difference normals (neuralangelo-dtu-wmask) on CUDA")
         import math
         n_rays, dev = rays.shape[0], rays.device
         cap = int(cfg.get('static_sample_capacity', 1 << 19))
@@ -202,7 +204,10 @@ class NeuSModel(BaseModel):
         ri32, t_starts, t_ends, offsets, k_dev = m['ray_indices'], m['t_starts'][:, None], m['t_ends'][:, None], m['offsets'], m['k_dev']
         with ops.live_rows(k_dev):
             positions, t_dirs, dists = ops.sample_points(rays, ri32, t_starts, t_ends)
-            sdf, sdf_grad, feature = self.geometry(positions, with_grad=True, with_feature=True)
+            if fd:
+                sdf, sdf_grad, feature, sdf_laplace = self.geometry(positions, with_grad=True, with_feature=True, with_laplace=True)
+            else:
+                sdf, sdf_grad, feature = self.geometry(positions, with_grad=True, with_feature=True)
             inv_s = self.variance.inv_s.clip(1e-6, 1e6).reshape(1)
             if self._cos_dev is None or self._cos_dev.device != dev:
                 self._cos_dev = torch.full((1,), float(self.cos_anneal_ratio), device=dev)
@@ -215,6 +220,8 @@ class NeuSModel(BaseModel):
         out = {'comp_rgb': comp_rgb, 'comp_normal': comp_normal, 'opacity': opacity, 'depth': depth, 'rays_valid': valid, 'num_samples': num,
                'sdf_samples': sdf, 'sdf_grad_samples': sdf_grad, 'weights': weights, 'points': ((t_starts + t_ends) / 2.).view(-1),
                'intervals': dists.view(-1), 'ray_indices': ri32, 'num_samples_dev': k_dev, 'overflow': m['overflow']}
+        if fd:
+            out['sdf_laplace_samples'] = sdf_laplace
         bg = self.background_color[None, :].expand(*comp_rgb.shape)
         out.update({'comp_rgb_bg': bg, 'num_samples_bg': torch.zeros_like(num), 'rays_valid_bg': torch.zeros_like(valid),
                     'comp_rgb_full': comp_rgb + bg * (1.0 - opacity), 'num_samples_full': num, 'rays_valid_full': valid})

@@ -521,6 +521,52 @@ def neus_sdf(spec, radius, points, table_f32, table_h, W1, b1, W2, b2):
                           contig(W1, torch.float32), contig(b1, torch.float32), contig(W2, torch.float32), contig(b2, torch.float32))
 
 
+class _NeusSDFFd(torch.autograd.Function):
+    """(sdf, grad, feature, laplace) = VolumeSDF.forward(points, with_laplace=True) with finite-difference normals
+    (models/geometry.py:181-199): the centre and the six stencil evaluations in one kernel, their first-order backward in another."""
+
+    @staticmethod
+    def forward(ctx, spec, radius, n_out, stencil, points, table_f32, table_h, W1, b1, W2, b2, fd_state):
+        n = points.shape[0]
+        dev = points.device
+        sdf = torch.empty(n, device=dev)
+        feat = torch.empty(n, n_out, device=dev)
+        grad = torch.empty(n, 3, device=dev) if stencil else None
+        lap = torch.empty(n, device=dev) if stencil else None
+        lib.call('nsr_neus_field_fd_fwd', spec.ref(), ptr(points), ptr(table_h), ptr(W1), ptr(b1), ptr(W2), ptr(b2), float(radius), int(n_out),
+                 ptr(fd_state), ptr(sdf), ptr(grad), ptr(feat), ptr(lap), n, ptr(_LIVE_ROWS), stream())
+        ctx.spec, ctx.radius, ctx.n_out, ctx.k_dev = spec, radius, n_out, _LIVE_ROWS
+        ctx.save_for_backward(points, table_h, W1, b1, W2, b2, fd_state)
+        return sdf, grad, feat, lap
+
+    @staticmethod
+    def backward(ctx, g_sdf, g_grad, g_feat, g_lap):
+        points, table_h, W1, b1, W2, b2, fd_state = ctx.saved_tensors
+        n, dev = points.shape[0], points.device
+        g_sdf, g_grad, g_feat, g_lap = (contig(t, torch.float32) for t in (g_sdf, g_grad, g_feat, g_lap))
+        dtable = torch.zeros(ctx.spec.n_params, device=dev)
+        sizes = [W1.numel(), b1.numel(), W2.numel(), b2.numel()]
+        flat = torch.zeros(sum(sizes), device=dev)   # one fill for the four small gradients
+        dW1, db1, dW2, db2 = [t.view_as(w) for t, w in zip(flat.split(sizes), (W1, b1, W2, b2))]
+        lib.call('nsr_neus_field_fd_bwd', ctx.spec.ref(), ptr(points), ptr(table_h), ptr(W1), ptr(b1), ptr(W2), ptr(b2), float(ctx.radius),
+                 int(ctx.n_out), ptr(fd_state), ptr(g_feat), ptr(g_sdf), ptr(g_grad), ptr(g_lap), ptr(dtable), ptr(dW1), ptr(db1), ptr(dW2),
+                 ptr(db2), n, ptr(ctx.k_dev), stream())
+        return None, None, None, None, None, dtable, None, dW1, db1, dW2, db2, None
+
+
+def neus_sdf_fd(spec, radius, points, table_f32, table_h, W1, b1, W2, b2, fd_state, with_grad=True):
+    """points [N,3] world (AABB scene of half-extent `radius`); weights as in neus_sdf; fd_state: float32 [3] CUDA tensor
+    {eps, eps^2, n_active} (hash levels >= n_active give 0).  -> (sdf [N], grad [N,3], feature [N,n_out], laplace [N]);
+    with_grad=False evaluates the centre only and returns grad = laplace = None."""
+    check_cuda(points, table_h, W1, W2, fd_state, what='VolumeSDF (fused, finite difference)')
+    if fd_state.dtype != torch.float32 or fd_state.numel() != 3 or not fd_state.is_contiguous():
+        raise ValueError('fd_state must be a contiguous float32 tensor of 3 entries {eps, eps^2, n_active}')
+    n_out = W2.shape[0]
+    return _NeusSDFFd.apply(spec, float(radius), int(n_out), bool(with_grad), contig(points.detach(), torch.float32), table_f32, table_h,
+                            contig(W1, torch.float32), contig(b1, torch.float32), contig(W2, torch.float32), contig(b2, torch.float32),
+                            fd_state)
+
+
 # --------------------------------------------------------------------------------------------------
 # NeuS shading: SDF -> alpha (+ normal), compositing, fused VolumeRadiance
 # --------------------------------------------------------------------------------------------------
