@@ -68,6 +68,9 @@ typedef struct {
   int32_t feature_dim;     /* must be 16 */
   int32_t density_hidden;  /* must be 1 */
   int32_t color_hidden;    /* must be 2 */
+  int32_t contraction;     /* 0 AABB (above), 2 UN_BOUNDED_SPHERE: x01 -> v = 2 x01 - 1, |v| > 1 -> (2 - 1/|v|) v/|v|, then v/4 + 1/2
+                              (models/geometry.py contract_to_unisphere); honoured by nsr_nerf_density / _prepass / _render_fwd /
+                              nsr_nerf_field_bwd without xyzdir; every other entry point needs 0 */
 } nsr_nerf_t;
 
 /* VolumeRadiance fused kernel (models/texture.py:23-30): input = cat[feature (n_feat) | SH degree 4 of the ray direction (16) |
@@ -200,6 +203,19 @@ int nsr_march_rays_mask(const nsr_march_t* p, const float* rays, const float* ji
 int nsr_scan_counts_order(const int32_t* counts, int64_t* offsets, int32_t* order, int64_t n, void* stream);
 int nsr_march_rays_expand(const nsr_march_t* p, const uint32_t* masks, int32_t words, const float* t_min, const int64_t* offsets,
                           int32_t* ray_indices, float* t_starts, float* t_ends, int64_t n_rays, void* stream);
+/* marching for the unbounded fused path (cone_angle > 0, any contraction; same sample sets as nsr_march_count/_write given the same
+ * intervals): one warp per ray; every lane runs the same fp32 step recurrence t1 = t0 + min(max(t0 * cone, step), 1e10) for a 32-step
+ * chunk and lane k tests step k against the bitfield.  Per-ray interval in nerfacc's order: t_min = max(t_min_in[ray] or 0, near),
+ * t_max = min(t_max_in[ray] or 1e10, far), then t_min += jitter[ray] * step when jitter != NULL (t_min_in / t_max_in / jitter may be
+ * NULL; pass near = -inf / far = +inf for none).  nsr_march_cone_mask writes per-ray masks [n_rays, words] (words * 32 = the step bound of
+ * a ray: it never takes more steps), the per-ray counts and the ray's first t (t_start [n_rays]); nsr_scan_counts turns the counts into
+ * ray-ordered offsets.  nsr_march_cone_expand recomputes the recurrence and writes packed samples at offsets; rows at or past cap are
+ * not written, and a ray reaching past cap sets *overflow (device int32, may be NULL) to 1. */
+int nsr_march_cone_mask(const nsr_march_t* p, const float* rays, const float* jitter, const float* t_min_in, const float* t_max_in, float near,
+                        float far, const uint32_t* bits, uint32_t* masks, int32_t words, float* t_start, int32_t* counts, int64_t n_rays,
+                        void* stream);
+int nsr_march_cone_expand(const nsr_march_t* p, const uint32_t* masks, int32_t words, const float* t_start, const int64_t* offsets,
+                          int32_t* ray_indices, float* t_starts, float* t_ends, int64_t cap, int32_t* overflow, int64_t n_rays, void* stream);
 /* density at world positions (occ_eval_fn of models/nerf.py:49-52; VolumeDensity.forward density-only).
  * positions f32 [n,3]; dparams fp16 flat [3072 MLP | table]; density f32 [n]. */
 int nsr_nerf_density(const nsr_nerf_t* f, const float* positions, const void* dparams_h, float* density, int64_t n, void* stream);

@@ -289,6 +289,95 @@ __global__ void __launch_bounds__(kMarchWarps * 32) march_rays_expand_kernel(nsr
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Fused-path marcher for cone_angle > 0 (unbounded scenes): march_seq_kernel's serial recurrence, one warp per ray.  The step
+// t1 = t0 + min(max(t0 * cone, step), 1e10) depends on the previous one, so it is not reassociated: every lane runs the SAME fp32
+// chain over a 32-step chunk (arithmetic only, no loads) and lane k keeps step k; the 32 occupancy tests of a chunk -- the loads --
+// then run in parallel.  The expand pass recomputes the chain instead of storing t per chunk.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float cone_next(float t0, float cone, float step) { return t0 + fminf(fmaxf(t0 * cone, step), 1e10f); }
+
+// advance the chain by 32 steps from t (chunk start); lane `lane` receives its step [t0, t1)
+__device__ __forceinline__ float cone_chunk(float t, float cone, float step, int lane, float& t0, float& t1) {
+#pragma unroll
+  for (int k = 0; k < 32; ++k) {
+    const float tn = cone_next(t, cone, step);
+    if (k == lane) {
+      t0 = t;
+      t1 = tn;
+    }
+    t = tn;
+  }
+  return t;
+}
+
+__global__ void __launch_bounds__(kMarchWarps * 32) march_cone_mask_kernel(nsr_march_t p, const float* __restrict__ rays,
+                                                                           const float* __restrict__ jitter, const float* __restrict__ t_min_in,
+                                                                           const float* __restrict__ t_max_in, float near, float far,
+                                                                           const uint32_t* __restrict__ bits, uint32_t* __restrict__ masks,
+                                                                           int words, float* __restrict__ t_start, int32_t* __restrict__ counts,
+                                                                           int64_t n_rays) {
+  const int lane = threadIdx.x & 31;
+  const int64_t ray = blockIdx.x * (int64_t)kMarchWarps + (threadIdx.x >> 5);
+  if (ray >= n_rays) return;
+  const float* rr = rays + ray * 6;
+  const float ox = rr[0], oy = rr[1], oz = rr[2], dx = rr[3], dy = rr[4], dz = rr[5];
+  const float step = p.step, cone = p.cone_angle;
+  // nerfacc.ray_marching's order: interval (or [0, 1e10)), clamp to the near / far planes, then the stratified offset (unfused mul, add)
+  float tmin = fmaxf(t_min_in ? t_min_in[ray] : 0.f, near);
+  const float tmax = fminf(t_max_in ? t_max_in[ray] : 1e10f, far);
+  if (jitter != nullptr) tmin = tmin + jitter[ray] * step;
+  uint32_t* mrow = masks + ray * words;
+  float t = tmin;
+  int cnt = 0;
+  for (int w = 0; w < words; ++w) {
+    float t0 = 0.f, t1 = 0.f;
+    t = cone_chunk(t, cone, step, lane, t0, t1);
+    const float tm = (t0 + t1) * 0.5f;
+    const bool valid = tm < tmax;
+    const bool occ = valid && occupied(p, bits, __fmaf_rn(tm, dx, ox), __fmaf_rn(tm, dy, oy), __fmaf_rn(tm, dz, oz));
+    const uint32_t m = __ballot_sync(0xffffffffu, occ);
+    if (lane == 0) mrow[w] = m;
+    cnt += __popc(m);
+    if (!__shfl_sync(0xffffffffu, (int)valid, 31)) break;  // tm is monotone along the ray; words past here are never read
+  }
+  if (lane == 0) {
+    counts[ray] = cnt;
+    t_start[ray] = tmin;
+  }
+}
+
+__global__ void __launch_bounds__(kMarchWarps * 32) march_cone_expand_kernel(nsr_march_t p, const uint32_t* __restrict__ masks, int words,
+                                                                             const float* __restrict__ t_start,
+                                                                             const int64_t* __restrict__ offsets, int32_t* __restrict__ ray_indices,
+                                                                             float* __restrict__ t_starts, float* __restrict__ t_ends, int64_t cap,
+                                                                             int32_t* __restrict__ overflow, int64_t n_rays) {
+  const int lane = threadIdx.x & 31;
+  const int64_t ray = blockIdx.x * (int64_t)kMarchWarps + (threadIdx.x >> 5);
+  if (ray >= n_rays) return;
+  const int64_t beg = offsets[ray], end = offsets[ray + 1];
+  if (end <= beg) return;
+  if (end > cap && overflow != nullptr && lane == 0) *overflow = 1;
+  const float step = p.step, cone = p.cone_angle;
+  const uint32_t* mrow = masks + ray * words;
+  float t = t_start[ray];
+  int64_t base = beg;
+  for (int w = 0; w < words && base < end && base < cap; ++w) {
+    float t0 = 0.f, t1 = 0.f;
+    t = cone_chunk(t, cone, step, lane, t0, t1);
+    const uint32_t m = mrow[w];
+    if ((m >> lane) & 1u) {
+      const int64_t pos = base + __popc(m & ((1u << lane) - 1u));
+      if (pos < cap) {
+        ray_indices[pos] = (int32_t)ray;
+        t_starts[pos] = t0;
+        t_ends[pos] = t1;
+      }
+    }
+    base += __popc(m);
+  }
+}
+
 template <bool WRITE>
 int launch_march(const nsr_march_t* p, const float* rays_o, const float* rays_d, const float* t_min, const float* t_max,
                  const uint32_t* bits, int32_t* counts, const int64_t* offsets, int32_t* ray_indices, float* t_starts, float* t_ends,
@@ -392,6 +481,35 @@ extern "C" int nsr_march_rays_expand(const nsr_march_t* p, const uint32_t* masks
                                                                                                            ray_indices, t_starts, t_ends,
                                                                                                            n_rays);
   NSR_CHECK_LAUNCH("nsr_march_rays_expand");
+  return 0;
+}
+
+extern "C" int nsr_march_cone_mask(const nsr_march_t* p, const float* rays, const float* jitter, const float* t_min_in, const float* t_max_in,
+                                   float near, float far, const uint32_t* bits, uint32_t* masks, int32_t words, float* t_start, int32_t* counts,
+                                   int64_t n_rays, void* stream) {
+  NSR_REQUIRE(p != nullptr, "nsr_march_cone_mask: march descriptor is NULL");
+  NSR_REQUIRE(p->res >= 1 && p->res <= 1024, "nsr_march_cone_mask: grid resolution %d out of range", p->res);
+  NSR_REQUIRE(p->contraction == 0 || p->contraction == 2, "nsr_march_cone_mask: contraction type %d not implemented (AABB=0, UN_BOUNDED_SPHERE=2)",
+              p->contraction);
+  NSR_REQUIRE(p->step > 0.f && p->cone_angle >= 0.f, "nsr_march_cone_mask: needs step > 0 and cone_angle >= 0");
+  NSR_REQUIRE(words >= 1, "nsr_march_cone_mask: words must be >= 1");
+  NSR_REQUIRE(rays != nullptr && bits != nullptr && masks != nullptr && t_start != nullptr && counts != nullptr, "nsr_march_cone_mask: NULL argument");
+  if (n_rays == 0) return 0;
+  march_cone_mask_kernel<<<nsr_blocks(n_rays, kMarchWarps), kMarchWarps * 32, 0, (cudaStream_t)stream>>>(
+      *p, rays, jitter, t_min_in, t_max_in, near, far, bits, masks, words, t_start, counts, n_rays);
+  NSR_CHECK_LAUNCH("nsr_march_cone_mask");
+  return 0;
+}
+
+extern "C" int nsr_march_cone_expand(const nsr_march_t* p, const uint32_t* masks, int32_t words, const float* t_start, const int64_t* offsets,
+                                     int32_t* ray_indices, float* t_starts, float* t_ends, int64_t cap, int32_t* overflow, int64_t n_rays,
+                                     void* stream) {
+  NSR_REQUIRE(p != nullptr && p->step > 0.f, "nsr_march_cone_expand: descriptor is NULL or step <= 0");
+  NSR_REQUIRE(words >= 1 && cap >= 0, "nsr_march_cone_expand: needs words >= 1 and cap >= 0");
+  if (n_rays == 0) return 0;
+  march_cone_expand_kernel<<<nsr_blocks(n_rays, kMarchWarps), kMarchWarps * 32, 0, (cudaStream_t)stream>>>(
+      *p, masks, words, t_start, offsets, ray_indices, t_starts, t_ends, cap, overflow, n_rays);
+  NSR_CHECK_LAUNCH("nsr_march_cone_expand");
   return 0;
 }
 

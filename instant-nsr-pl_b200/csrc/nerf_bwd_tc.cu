@@ -528,8 +528,8 @@ extern "C" int nsr_nerf_field_bwd_tc(const nsr_nerf_t* f, const void* enc_tiles_
                                      const float* d_sraw, const float* d_rgb, float* grad_dparams, float* grad_cparams, float loss_scale,
                                      const float* amax, int64_t k, const int64_t* k_dev, const float* xyzdir, int* status, void* stream) {
   NSR_REQUIRE(f != nullptr, "nsr_nerf_field_bwd_tc: field descriptor is NULL");
-  NSR_REQUIRE(f->grid.n_levels == 16 && f->grid.n_features == 2 && f->feature_dim == 16 && f->density_hidden == 1 && f->color_hidden == 2,
-              "nsr_nerf_field_bwd_tc: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2");
+  NSR_REQUIRE(f->grid.n_levels == 16 && f->grid.n_features == 2 && f->feature_dim == 16 && f->density_hidden == 1 && f->color_hidden == 2 && f->contraction == 0,
+              "nsr_nerf_field_bwd_tc: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2, AABB contraction");
   NSR_REQUIRE(loss_scale > 0.f || amax != nullptr, "nsr_nerf_field_bwd_tc: loss_scale <= 0 (automatic) needs the amax pointer");
   NSR_REQUIRE(enc_tiles_h != nullptr && xyzdir != nullptr && d_sraw != nullptr && d_rgb != nullptr, "nsr_nerf_field_bwd_tc: NULL input");
   if (k == 0) return 0;

@@ -28,17 +28,54 @@ __device__ __forceinline__ void nf_stage_weights(__half* smem, const __half* __r
   }
 }
 
+// contraction codes of nsr_nerf_t::contraction (nerfacc.ContractionType)
+constexpr int NF_AABB = 0;
+constexpr int NF_UNBOUNDED_SPHERE = 2;
+
+// world position -> [0,1]^3 under UN_BOUNDED_SPHERE, in the op order of contract_to_unisphere (models/fields.py): scale to [0,1]
+// (add, true division), v = 2u - 1, |v| > 1 -> (2 - 1/|v|) * (v / |v|), v/4 + 1/2
+__device__ __forceinline__ void nf_contract_sphere(float radius, float& x, float& y, float& z) {
+  const float span = 2.f * radius;
+  float vx = __fsub_rn(__fmul_rn(__fdiv_rn(__fadd_rn(x, radius), span), 2.f), 1.f);
+  float vy = __fsub_rn(__fmul_rn(__fdiv_rn(__fadd_rn(y, radius), span), 2.f), 1.f);
+  float vz = __fsub_rn(__fmul_rn(__fdiv_rn(__fadd_rn(z, radius), span), 2.f), 1.f);
+  const float mag = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(vx, vx), __fmul_rn(vy, vy)), __fmul_rn(vz, vz)));
+  if (mag > 1.f) {
+    const float s = __fsub_rn(2.f, __fdiv_rn(1.f, mag));
+    vx = __fmul_rn(s, __fdiv_rn(vx, mag));
+    vy = __fmul_rn(s, __fdiv_rn(vy, mag));
+    vz = __fmul_rn(s, __fdiv_rn(vz, mag));
+  }
+  x = __fadd_rn(__fmul_rn(vx, 0.25f), 0.5f);
+  y = __fadd_rn(__fmul_rn(vy, 0.25f), 0.5f);
+  z = __fadd_rn(__fmul_rn(vz, 0.25f), 0.5f);
+}
+
+// world position -> unit-cube position of the field (contract_to_unisphere: models/geometry.py:17-19)
+template <int CT>
+__device__ __forceinline__ void nf_contract(const nsr_nerf_t& P, float& x, float& y, float& z) {
+  if (CT == NF_UNBOUNDED_SPHERE) {
+    nf_contract_sphere(P.radius, x, y, z);
+  } else {
+    const float inv = 1.f / (2.f * P.radius);
+    x = (x + P.radius) * inv;
+    y = (y + P.radius) * inv;
+    z = (z + P.radius) * inv;
+  }
+}
+
 // sample (ray, t0, t1) -> unit-cube position (contract_to_unisphere, AABB: models/geometry.py:17-19)
+template <int CT = NF_AABB>
 __device__ __forceinline__ void nf_sample_position(const nsr_nerf_t& P, const float* __restrict__ rays, int ray, float t0, float t1,
                                                    float& x, float& y, float& z, float& dx, float& dy, float& dz) {
   const float* r = rays + (size_t)ray * 6;
   const float ox = __ldg(r + 0), oy = __ldg(r + 1), oz = __ldg(r + 2);
   dx = __ldg(r + 3); dy = __ldg(r + 4); dz = __ldg(r + 5);
   const float mid = (t0 + t1) * 0.5f;
-  const float inv = 1.f / (2.f * P.radius);
-  x = (fmaf(dx, mid, ox) + P.radius) * inv;
-  y = (fmaf(dy, mid, oy) + P.radius) * inv;
-  z = (fmaf(dz, mid, oz) + P.radius) * inv;
+  x = fmaf(dx, mid, ox);
+  y = fmaf(dy, mid, oy);
+  z = fmaf(dz, mid, oz);
+  nf_contract<CT>(P, x, y, z);
 }
 
 // x-adjacent corner pair (i0 = x bit 0, i1 = x bit 1) of one (y,z) combination.

@@ -87,7 +87,8 @@ __device__ __forceinline__ void relu_mask_pack(const float (&acc)[1][8][4], cons
 // into the second smem buffer while tile t computes: no load of the kernel sits in front of the math any more (ncu before:
 // 37 % of the stall samples were long-scoreboard waits on the row_pos -> enc / ray_indices -> rays chains and on the tile's loads).
 // The split backward (d(encoding) to memory, REDs in a separate kernel) uses nerf_bwd_net_kernel below instead.
-template <bool PACKED>
+// CT: the field's contraction (NF_AABB / NF_UNBOUNDED_SPHERE) of the positions recomputed from the rays (!PACKED; xyzdir is AABB-only)
+template <bool PACKED, int CT>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __grid_constant__ nsr_nerf_t P, const float* __restrict__ rays,
                                                                const int32_t* __restrict__ ray_indices, const float* __restrict__ t_starts,
                                                                const float* __restrict__ t_ends, const __half* __restrict__ enc_save,
@@ -293,7 +294,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
           y = rr[1];
           z = rr[2];
         } else {
-          nf_sample_position(P, rays, ray_indices[i], t_starts[i], t_ends[i], x, y, z, dx, dy, dz);
+          nf_sample_position<CT>(P, rays, ray_indices[i], t_starts[i], t_ends[i], x, y, z, dx, dy, dz);
         }
       }
 #pragma unroll
@@ -767,10 +768,14 @@ int field_bwd_launch(const nsr_nerf_t* f, const float* rays, const int32_t* ray_
   NSR_REQUIRE(loss_scale > 0.f || amax != nullptr, "%s: loss_scale <= 0 (automatic) needs the amax pointer", who);
   if (k == 0) return 0;
   NSR_REQUIRE(xyzdir == nullptr || row_pos == nullptr, "%s: packed inputs (xyzdir) and row_pos are mutually exclusive", who);
+  NSR_REQUIRE(f->contraction == NF_AABB || (f->contraction == NF_UNBOUNDED_SPHERE && xyzdir == nullptr),
+              "%s: contraction type %d not implemented here (AABB=0; UN_BOUNDED_SPHERE=2 only without xyzdir)", who, f->contraction);
   static thread_local bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(nerf_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(nerf_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(nerf_bwd_kernel<false, NF_AABB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(nerf_bwd_kernel<true, NF_AABB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(nerf_bwd_kernel<false, NF_UNBOUNDED_SPHERE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e != cudaSuccess) {
       nsr_set_error("%s: cannot reserve %zu B shared memory: %s", who, kSmemBytes, cudaGetErrorString(e));
       return 2;
@@ -784,9 +789,11 @@ int field_bwd_launch(const nsr_nerf_t* f, const float* rays, const int32_t* ray_
   *f, rays, ray_indices, t_starts, t_ends, (const __half*)enc_save_h, (const __half*)dparams_h, (const __half*)cparams_h, d_sraw, d_rgb,    \
       grad_dparams, grad_cparams, loss_scale, amax, k, k_dev, row_pos, xyzdir
   if (xyzdir != nullptr)
-    nerf_bwd_kernel<true><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
+    nerf_bwd_kernel<true, NF_AABB><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
+  else if (f->contraction == NF_UNBOUNDED_SPHERE)
+    nerf_bwd_kernel<false, NF_UNBOUNDED_SPHERE><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
   else
-    nerf_bwd_kernel<false><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
+    nerf_bwd_kernel<false, NF_AABB><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
 #undef NSR_BWD_ARGS
   NSR_CHECK_LAUNCH(who);
   return 0;
@@ -801,6 +808,7 @@ int field_bwd_net_launch(const nsr_nerf_t* f, const void* enc_k_h, const void* d
               "%s: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2", who);
   NSR_REQUIRE(loss_scale > 0.f || amax != nullptr, "%s: loss_scale <= 0 (automatic) needs the amax pointer", who);
   NSR_REQUIRE(denc_h != nullptr && xyzdir != nullptr, "%s: denc / xyzdir is NULL", who);
+  NSR_REQUIRE(f->contraction == NF_AABB, "%s: packed inputs (xyzdir) need the AABB contraction (got %d)", who, f->contraction);
   if (k == 0) return 0;
   static thread_local bool attr_set = false;
   if (!attr_set) {

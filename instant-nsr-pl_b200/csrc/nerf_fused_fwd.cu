@@ -35,7 +35,8 @@ struct FwdArgs {
   const int64_t* n_dev;       // optional: the count lives on the device (no host sync / graph capture)
 };
 
-template <int MODE>
+// CT: the field's contraction (NF_AABB / NF_UNBOUNDED_SPHERE), a template parameter so that the AABB build is unchanged
+template <int MODE, int CT>
 __global__ void __launch_bounds__(kThreads, 2) nerf_fwd_kernel(const __grid_constant__ nsr_nerf_t P, const FwdArgs a) {
   extern __shared__ __align__(16) __half smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
@@ -56,15 +57,15 @@ __global__ void __launch_bounds__(kThreads, 2) nerf_fwd_kernel(const __grid_cons
     int ray = -1;
     if (valid) {
       if (MODE == MODE_DENSITY) {
-        const float inv = 1.f / (2.f * P.radius);
-        x = (a.positions[i * 3 + 0] + P.radius) * inv;
-        y = (a.positions[i * 3 + 1] + P.radius) * inv;
-        z = (a.positions[i * 3 + 2] + P.radius) * inv;
+        x = a.positions[i * 3 + 0];
+        y = a.positions[i * 3 + 1];
+        z = a.positions[i * 3 + 2];
+        nf_contract<CT>(P, x, y, z);
       } else {
         ray = a.ray_indices[i];
         t0 = a.t_starts[i];
         t1 = a.t_ends[i];
-        nf_sample_position(P, a.rays, ray, t0, t1, x, y, z, dx, dy, dz);
+        nf_sample_position<CT>(P, a.rays, ray, t0, t1, x, y, z, dx, dy, dz);
       }
     }
     uint32_t f[16];
@@ -277,16 +278,16 @@ int check_nerf(const nsr_nerf_t* f, const char* name) {
   NSR_REQUIRE(f->feature_dim == 16 && f->density_hidden == 1 && f->color_hidden == 2,
               "%s: fused path needs feature_dim=16, 1 density hidden layer, 2 colour hidden layers", name);
   NSR_REQUIRE(f->radius > 0.f, "%s: radius must be > 0", name);
+  NSR_REQUIRE(f->contraction == NF_AABB || f->contraction == NF_UNBOUNDED_SPHERE,
+              "%s: contraction type %d not implemented (AABB=0, UN_BOUNDED_SPHERE=2)", name, f->contraction);
   return 0;
 }
 
-template <int MODE>
-int launch_fwd(const nsr_nerf_t* f, const FwdArgs& a, cudaStream_t st, const char* name) {
-  if (int e = check_nerf(f, name)) return e;
-  if (a.n == 0) return 0;
+template <int MODE, int CT>
+int launch_fwd_ct(const nsr_nerf_t* f, const FwdArgs& a, cudaStream_t st, const char* name) {
   static thread_local bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(nerf_fwd_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(nerf_fwd_kernel<MODE, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e != cudaSuccess) {
       nsr_set_error("%s: cannot reserve %zu B shared memory: %s", name, kSmemBytes, cudaGetErrorString(e));
       return 2;
@@ -297,9 +298,17 @@ int launch_fwd(const nsr_nerf_t* f, const FwdArgs& a, cudaStream_t st, const cha
   int grid = (int)min((int64_t)nsr_sm_count() * 2, (tiles + kWarps - 1) / kWarps);
   if (grid < 1) grid = 1;
   if (a.n_dev != nullptr) grid = nsr_sm_count() * 2;  // count unknown on the host: full persistent grid
-  nerf_fwd_kernel<MODE><<<grid, kThreads, kSmemBytes, st>>>(*f, a);
+  nerf_fwd_kernel<MODE, CT><<<grid, kThreads, kSmemBytes, st>>>(*f, a);
   NSR_CHECK_LAUNCH(name);
   return 0;
+}
+
+template <int MODE>
+int launch_fwd(const nsr_nerf_t* f, const FwdArgs& a, cudaStream_t st, const char* name) {
+  if (int e = check_nerf(f, name)) return e;
+  if (a.n == 0) return 0;
+  if (f->contraction == NF_UNBOUNDED_SPHERE) return launch_fwd_ct<MODE, NF_UNBOUNDED_SPHERE>(f, a, st, name);
+  return launch_fwd_ct<MODE, NF_AABB>(f, a, st, name);
 }
 
 }  // namespace

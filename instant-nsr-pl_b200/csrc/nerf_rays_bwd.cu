@@ -420,8 +420,8 @@ extern "C" int nsr_nerf_rays_bwd(const nsr_nerf_t* f, const float* rays, const f
                                  float* grad_cparams, float loss_scale, float* amax, float t_bound, uint32_t* ticket, int64_t n_rays,
                                  void* stream) {
   NSR_REQUIRE(f != nullptr && f->grid.n_levels == 16 && f->grid.n_features == 2 && f->feature_dim == 16 && f->density_hidden == 1 &&
-                  f->color_hidden == 2,
-              "nsr_nerf_rays_bwd: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2");
+                  f->color_hidden == 2 && f->contraction == 0,
+              "nsr_nerf_rays_bwd: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2, AABB contraction");
   NSR_REQUIRE(ticket != nullptr && amax != nullptr, "nsr_nerf_rays_bwd: ticket and amax (device scalars, zeroed) are required");
   if (n_rays == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;

@@ -421,8 +421,8 @@ extern "C" int nsr_nerf_rays_fwd(const nsr_nerf_t* f, const float* rays, const u
                                  const int32_t* counts, const int32_t* bin_counts, int32_t* kept_blocks, void* stream) {
   NSR_REQUIRE(bin_counts == nullptr || (order != nullptr && counts != nullptr), "nsr_nerf_rays_fwd: the binned queue needs order [8][n] and counts");
   NSR_REQUIRE(f != nullptr && f->grid.n_levels == 16 && f->grid.n_features == 2 && f->feature_dim == 16 && f->density_hidden == 1 &&
-                  f->color_hidden == 2,
-              "nsr_nerf_rays_fwd: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2");
+                  f->color_hidden == 2 && f->contraction == 0,
+              "nsr_nerf_rays_fwd: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2, AABB contraction");
   NSR_REQUIRE(words >= 1 && words <= kMaxWords, "nsr_nerf_rays_fwd: words must be in [1,%d]", kMaxWords);
   NSR_REQUIRE(ticket != nullptr && kept != nullptr, "nsr_nerf_rays_fwd: ticket / kept are required");
   if (n_rays == 0) return 0;

@@ -29,8 +29,8 @@ class _NerfRender(torch.autograd.Function):
     """(dparams, cparams) -> per-ray sums + per-sample weights; everything else rides along non-differentiably."""
 
     @staticmethod
-    def forward(ctx, dparams, cparams, fused, rays, jitter):
-        st = fused.trace(rays, jitter)
+    def forward(ctx, dparams, cparams, fused, rays, jitter, static=False):
+        st = fused.trace(rays, jitter, static)
         n_rays, cap = rays.shape[0], st['cap']
         dev = rays.device
         acc_rgb = torch.zeros(n_rays, 3, device=dev)
@@ -49,8 +49,8 @@ class _NerfRender(torch.autograd.Function):
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(rays, st['ri'], st['ts'], st['te'], st['trans'], st['offsets_k'], enc, sig, rgbs, weights, dh, ch)
         counts = torch.cat([st['offsets_m'][n_rays:], k_dev])  # [M, K] on the device
-        ctx.mark_non_differentiable(st['ri'], st['ts'], st['te'], counts)
-        return acc_rgb, opacity, depth, weights, st['ri'], st['ts'], st['te'], counts
+        ctx.mark_non_differentiable(st['ri'], st['ts'], st['te'], counts, *([st['overflow']] if st['overflow'] is not None else []))
+        return acc_rgb, opacity, depth, weights, st['ri'], st['ts'], st['te'], counts, st['overflow']
 
     @staticmethod
     def backward(ctx, g_rgb, g_op, g_depth, g_w, *_):
@@ -69,7 +69,7 @@ class _NerfRender(torch.autograd.Function):
                      ptr(f32(g_op)), ptr(f32(g_depth)), ptr(f32(g_w)), ptr(d_sraw), ptr(d_rgb), ptr(amax), n_rays, stream())
             lib.call('nsr_nerf_field_bwd', fused.ref(), ptr(rays), ptr(ri), ptr(ts), ptr(te), ptr(enc), ptr(dh), ptr(ch), ptr(d_sraw),
                      ptr(d_rgb), ptr(gd), ptr(gc), float(fused.loss_scale), ptr(amax), cap, ptr(offsets_k[n_rays:]), None, None, stream())
-        return gd, gc, None, None, None
+        return gd, gc, None, None, None, None
 
 
 class _NerfRenderRays(torch.autograd.Function):
@@ -217,7 +217,9 @@ class _NerfRenderRays(torch.autograd.Function):
 
 
 class NerfFused:
-    """Fused executor attached to a NeRFModel whose config has the nerf-blender shape."""
+    """Fused executor attached to a NeRFModel whose config has the nerf-blender shape: the AABB scene of nerf-blender, or (config key
+    ``fused_unbounded``) the unbounded scene of nerf-colmap -- UN_BOUNDED_SPHERE contraction, cone marching from the near to the far
+    plane, which always runs the two-pass pipeline."""
 
     def __init__(self, model):
         self.model = model
@@ -232,15 +234,27 @@ class NerfFused:
         s.radius = r
         s.density_bias = float(geo.config.density_bias)
         s.feature_dim, s.density_hidden, s.color_hidden = 16, 1, 2
+        self.contracted = model.contraction_type == ContractionType.UN_BOUNDED_SPHERE
+        s.contraction = model.contraction_type.value
         self.struct = s
-        self.march = ops.march_struct([-r, -r, -r, r, r, r], model.occupancy_grid_res, ContractionType.AABB.value, model.render_step_size, 0.0)
-        # a ray crosses at most the box diagonal: upper bound on marched samples per ray (capacity of the static buffers)
-        self.cap_per_ray = int(math.ceil(2.0 * math.sqrt(3.0) * r / model.render_step_size)) + 2
+        self.march = ops.march_struct([-r, -r, -r, r, r, r], model.occupancy_grid_res, model.contraction_type.value, model.render_step_size,
+                                      model.cone_angle)
+        if self.contracted:
+            # blind cone stepping from the near to the far plane: every ray takes at most the steps of the earliest start (jitter 0)
+            self.near, self.far = float(model.near_plane), float(model.far_plane)
+            self.cap_per_ray = ops.cone_step_bound(max(0.0, self.near), min(1e10, self.far), model.render_step_size, model.cone_angle)
+        else:
+            # a ray crosses at most the box diagonal: upper bound on marched samples per ray (capacity of the static buffers)
+            self.cap_per_ray = int(math.ceil(2.0 * math.sqrt(3.0) * r / model.render_step_size)) + 2
+        # static=True, contracted: rows of the sample buffers (None = n_rays * cap_per_ray, which never overflows); config
+        # static_sample_capacity overrides it.  A step whose samples do not fit sets out['overflow'].
+        self.static_capacity = model.config.get('static_sample_capacity', None)
         self.loss_scale = 0.0  # <= 0: chosen on the device from the incoming gradient magnitude
         self.early_stop_eps, self.alpha_thre = 1e-4, 0.0
         self.last_stats = {}
         self._ticket = None
-        self.mode = 'per_ray'   # 'per_ray' (persistent per-ray forward kernel) | 'two_pass' (pre-pass / compaction / sample-tile kernels)
+        # 'per_ray' (persistent per-ray forward kernel) | 'two_pass' (pre-pass / compaction / sample-tile kernels; the only one contracted)
+        self.mode = 'two_pass' if self.contracted else 'per_ray'
         self.lean_static_outputs = False   # static=True: skip the per-ray outputs the fused loss op produces itself (comp_rgb, rays_valid)
         self.packed_bwd_inputs = True   # tile backward reads its inputs in packed row order (written by nsr_pack_kept)
         from .config import experimental
@@ -270,7 +284,8 @@ class NerfFused:
         cfg = model.config
         geo, tex = model.geometry, model.texture
         try:
-            ok = (not cfg.learned_background and cfg.grid_prune and isinstance(geo, VolumeDensity) and isinstance(tex, VolumeRadiance)
+            # learned_background (nerf-colmap: contracted, cone-marched) is opt-in through the model config key fused_unbounded
+            ok = ((not cfg.learned_background or cfg.get('fused_unbounded', False)) and cfg.grid_prune and isinstance(geo, VolumeDensity) and isinstance(tex, VolumeRadiance)
                   and isinstance(geo.encoding_with_network, tcnn.NetworkWithInputEncoding)
                   and geo.encoding_with_network.grid.n_levels == 16 and geo.encoding_with_network.mlp.n_hidden == 1
                   and geo.n_output_dims == 16 and geo.config.get('density_activation') == 'trunc_exp'
@@ -312,10 +327,12 @@ class NerfFused:
         return out.reshape(positions.shape[:-1])
 
     @torch.no_grad()
-    def trace(self, rays, jitter=None):
+    def trace(self, rays, jitter=None, static=True):
         """march + sigma_fn visibility pre-pass + compaction: the ``with torch.no_grad(): ray_marching(...)`` block of
         models/nerf.py:82-93, without a host sync.  Buffers have capacity n_rays * cap_per_ray; the true counts
-        are offsets_m[n_rays] (marched) and offsets_k[n_rays] (kept) on the device."""
+        are offsets_m[n_rays] (marched) and offsets_k[n_rays] (kept) on the device.  Contracted: the cone marcher, with
+        capacity-length buffers when static (see static_capacity; 'overflow' flags dropped samples), else buffers of exactly
+        the marched count (one device->host read)."""
         m = self.model
         dev = rays.device
         n = rays.shape[0]
@@ -325,16 +342,25 @@ class NerfFused:
         if m.randomized:
             u = torch.rand(n, device=dev) if jitter is None else contig(jitter.to(dev), torch.float32)
         grid = m.occupancy_grid
-        bits, coarse = grid.bits(), grid.coarse_bits()
         i32 = lambda k: torch.empty(k, dtype=torch.int32, device=dev)
         f32 = lambda k: torch.empty(k, dtype=torch.float32, device=dev)
-        words = (self.cap_per_ray + 31) // 32
-        masks, t_min = i32(n * words), f32(n)
-        counts, offsets_m = i32(n), torch.empty(n + 1, dtype=torch.int64, device=dev)
-        lib.call('nsr_march_rays_mask', mref, ptr(rays), ptr(u), ptr(bits), ptr(coarse), ptr(masks), words, ptr(t_min), ptr(counts), n, stream())
-        lib.call('nsr_scan_counts', ptr(counts), ptr(offsets_m), n, stream())
-        ri_m, ts_m, te_m = i32(cap), f32(cap), f32(cap)
-        lib.call('nsr_march_rays_expand', mref, ptr(masks), words, ptr(t_min), ptr(offsets_m), ptr(ri_m), ptr(ts_m), ptr(te_m), n, stream())
+        overflow = None
+        if self.contracted:
+            if static and self.static_capacity is not None:
+                cap = int(self.static_capacity)
+            mc = ops.march_cone(self.march, rays, u, max(0.0, self.near), min(1e10, self.far), grid.bits(), self.cap_per_ray,
+                                cap=cap if static else None)
+            ri_m, ts_m, te_m, offsets_m, overflow = mc['ray_indices'], mc['t_starts'], mc['t_ends'], mc['offsets'], mc['overflow']
+            cap = ri_m.shape[0]
+        else:
+            bits, coarse = grid.bits(), grid.coarse_bits()
+            words = (self.cap_per_ray + 31) // 32
+            masks, t_min = i32(n * words), f32(n)
+            counts, offsets_m = i32(n), torch.empty(n + 1, dtype=torch.int64, device=dev)
+            lib.call('nsr_march_rays_mask', mref, ptr(rays), ptr(u), ptr(bits), ptr(coarse), ptr(masks), words, ptr(t_min), ptr(counts), n, stream())
+            lib.call('nsr_scan_counts', ptr(counts), ptr(offsets_m), n, stream())
+            ri_m, ts_m, te_m = i32(cap), f32(cap), f32(cap)
+            lib.call('nsr_march_rays_expand', mref, ptr(masks), words, ptr(t_min), ptr(offsets_m), ptr(ri_m), ptr(ts_m), ptr(te_m), n, stream())
         alphas = f32(cap)
         lib.call('nsr_nerf_prepass', self.ref(), ptr(rays), ptr(ri_m), ptr(ts_m), ptr(te_m), ptr(self.dparams_half()), ptr(alphas), cap,
                  ptr(offsets_m[n:]), stream())
@@ -346,7 +372,7 @@ class NerfFused:
         ri, ts, te, tr = i32(cap), f32(cap), f32(cap), f32(cap)
         lib.call('nsr_compact_prefix', ptr(offsets_m), ptr(offsets_k), ptr(ri_m), ptr(ts_m), ptr(te_m), ptr(trans), ptr(ri), ptr(ts), ptr(te),
                  ptr(tr), n, stream())
-        return {'ri': ri, 'ts': ts, 'te': te, 'trans': tr, 'offsets_m': offsets_m, 'offsets_k': offsets_k, 'cap': cap}
+        return {'ri': ri, 'ts': ts, 'te': te, 'trans': tr, 'offsets_m': offsets_m, 'offsets_k': offsets_k, 'cap': cap, 'overflow': overflow}
 
     def render(self, rays, jitter=None, static=False):
         """NeRFModel.forward_ (models/nerf.py:61-127) -> the reference's output dict.
@@ -357,6 +383,8 @@ class NerfFused:
         m = self.model
         check_cuda(rays, what='NeRFModel')
         rays = contig(rays, torch.float32)
+        if self.contracted and self.mode != 'two_pass':
+            raise ValueError(f"NerfFused: the contracted (unbounded) field runs the 'two_pass' pipeline only, not mode={self.mode!r}")
         if self.mode == 'two_pass':
             return self._render_two_pass(rays, jitter, static)
         self._want_grad = torch.is_grad_enabled()
@@ -393,13 +421,17 @@ class NerfFused:
 
     def _render_two_pass(self, rays, jitter, static):
         m = self.model
-        acc_rgb, opacity, depth, weights, ri, ts, te, counts = _NerfRender.apply(self.net.params, self.cnet.params, self, rays, jitter)
+        acc_rgb, opacity, depth, weights, ri, ts, te, counts, overflow = _NerfRender.apply(self.net.params, self.cnet.params, self, rays,
+                                                                                          jitter, static)
         comp_rgb = acc_rgb + m.background_color * (1.0 - opacity)
         out = {'comp_rgb': comp_rgb, 'opacity': opacity, 'depth': depth, 'rays_valid': opacity > 0,
                'num_samples': counts[1:].to(torch.int32)}
         if static:
             self.last_stats = {'counts_dev': counts}
             k = None
+            if self.contracted:
+                # acc_rgb: the pre-blend colour sum nsr_b200.losses.nerf_rgb_loss takes; overflow: samples past the capacity were dropped
+                out.update({'acc_rgb': acc_rgb, 'overflow': overflow.bool()})
         else:
             n_marched, k = counts.tolist()
             self.last_stats = {'n_marched': n_marched, 'n_kept': k}

@@ -40,7 +40,7 @@ class MarchT(C.Structure):
 class NerfT(C.Structure):
     """nsr_nerf_t: fused NeRF field description (hash grid + density MLP + SH4 + colour MLP)."""
     _fields_ = [('grid', GridT), ('radius', C.c_float), ('density_bias', C.c_float), ('feature_dim', C.c_int32),
-                ('density_hidden', C.c_int32), ('color_hidden', C.c_int32)]
+                ('density_hidden', C.c_int32), ('color_hidden', C.c_int32), ('contraction', C.c_int32)]
 
 
 class RadianceT(C.Structure):
@@ -89,6 +89,8 @@ _SIGNATURES = {
     'nsr_scan_counts_order': [P, P, P, I64, P],
     'nsr_march_rays_alloc': [P, P, P, P, P, P, I32, P, P, P, P, P, P, I64, P],
     'nsr_march_rays_expand': [P, P, I32, P, P, P, P, P, I64, P],
+    'nsr_march_cone_mask': [P, P, P, P, P, F32, F32, P, P, I32, P, P, I64, P],
+    'nsr_march_cone_expand': [P, P, I32, P, P, P, P, P, I64, P, I64, P],
     'nsr_nerf_rays_fwd': [P, P, P, I32, P, P, P, F32, F32, P, P, P, P, P, P, P, P, P, P, P, P, P, I64, P, P, P, P],
     'nsr_pack_kept': [P, P, P, F32, P, P, P, P, P, P, P, P, P, P, P, P, I32, I64, P],
     'nsr_pack_kept_scan': [P, P, P, P, F32, P, P, P, P, P, P, P, P, P, P, P, P, I32, I64, P, P],

@@ -4,7 +4,8 @@ names, buffers, ``forward(rays) -> dict`` keys, train/eval behaviour).
 Two execution paths, identical results up to fp16 tolerance:
   * fused   (default when the config is the nerf-blender shape: HashGrid F=2 + FullyFusedMLP-64 fields,
              SH4 directions, trunc_exp density, sigmoid colour, AABB): libnsr_b200's fused kernels
-             (``nsr_b200.fused``), one launch per stage instead of ~40 torch/tcnn/nerfacc kernels.
+             (``nsr_b200.fused``), one launch per stage instead of ~40 torch/tcnn/nerfacc kernels.  The unbounded
+             nerf-colmap shape (learned_background) takes it only with the config key ``fused_unbounded: true``.
   * composed: the per-op tcnn-/nerfacc-shaped modules in the order the reference calls them.
 """
 import math

@@ -364,6 +364,55 @@ def ray_aabb_intersect(rays_o, rays_d, aabb):
     return t_min, t_max
 
 
+def cone_step_bound(t_min, t_max, step, cone_angle):
+    """Steps the cone marcher takes on a ray starting at ``t_min`` (fp32 recurrence t1 = t0 + min(max(t0 * cone, step), 1e10), step
+    taken while its midpoint is < t_max, as in csrc/march.cu).  Every step grows with t0, so a ray that starts later never takes more:
+    with t_min = the earliest start (e.g. the near plane, jitter 0) this bounds every ray (2073 for nerf-colmap)."""
+    f = np.float32
+    step, cone, t_max = f(step), f(cone_angle), f(t_max)
+    t0 = f(t_min)
+    n = 0
+    with np.errstate(over='ignore'):
+        while n < (1 << 24):
+            t1 = f(t0 + np.fmin(np.fmax(f(t0 * cone), step), f(1e10)))
+            if not f(f(t0 + t1) * f(0.5)) < t_max:
+                break
+            n += 1
+            t0 = t1
+    return n
+
+
+def march_cone(mstruct, rays, jitter, near, far, bits, bound, t_min=None, t_max=None, cap=None):
+    """Sync-free cone marching (csrc/march.cu, nsr_march_cone_mask / _expand): rays [N,6]; per-ray interval max(t_min or 0, near) ..
+    min(t_max or 1e10, far), + jitter * step when jitter is given; ``bound`` = steps per ray (cone_step_bound).  cap=None: exact-size
+    outputs (one device->host read of the total); else capacity-length buffers whose rows past the live count are undefined, offsets
+    clamped to cap, and overflow (int32 [1] device flag) set when samples were dropped.
+    -> dict(ray_indices i32, t_starts, t_ends f32, offsets i64 [N+1], overflow)."""
+    import ctypes
+    check_cuda(rays, bits, what='march_cone')
+    rays = contig(rays.detach(), torch.float32)
+    n, dev = rays.shape[0], rays.device
+    words = max(1, (int(bound) + 31) // 32)
+    masks = torch.empty(n * words, dtype=torch.int32, device=dev)
+    t_start = torch.empty(n, device=dev)
+    counts = torch.empty(n, dtype=torch.int32, device=dev)
+    offsets = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    mref = ctypes.byref(mstruct)
+    f32 = lambda t: contig(t, torch.float32) if t is not None else None
+    lib.call('nsr_march_cone_mask', mref, ptr(rays), ptr(f32(jitter)), ptr(f32(t_min)), ptr(f32(t_max)), float(near), float(far), ptr(bits),
+             ptr(masks), words, ptr(t_start), ptr(counts), n, stream())
+    lib.call('nsr_scan_counts', ptr(counts), ptr(offsets), n, stream())
+    if cap is None:
+        cap = int(offsets[n].item())   # exact size (what nerfacc's ray_marching allocates, after the same host read)
+    overflow = torch.zeros(1, dtype=torch.int32, device=dev)
+    ri = torch.empty(cap, dtype=torch.int32, device=dev)
+    ts, te = torch.empty(cap, device=dev), torch.empty(cap, device=dev)
+    lib.call('nsr_march_cone_expand', mref, ptr(masks), words, ptr(t_start), ptr(offsets), ptr(ri), ptr(ts), ptr(te), cap, ptr(overflow), n,
+             stream())
+    offsets.clamp_(max=cap)
+    return {'ray_indices': ri, 't_starts': ts, 't_ends': te, 'offsets': offsets, 'overflow': overflow}
+
+
 def march(mstruct, rays_o, rays_d, t_min, t_max, bits):
     """-> ray_indices int32 [M], t_starts [M], t_ends [M], offsets int64 [N+1]."""
     import ctypes

@@ -132,6 +132,9 @@ class P2PGradSync:
     def bind_direct(self, fused):
         """let the fused NeRF backward accumulate straight into the symmetric buffer (NerfFused.direct_grads): no 50 MB copy-in per step.
         The backward then zeroes + fills the views itself and autograd is bypassed for these two parameters."""
+        if getattr(fused, 'contracted', False):
+            raise ValueError('P2PGradSync.bind_direct / bind_pipelined serve the per-ray fused NeRF backward only; the unbounded (contracted, '
+                             'two-pass) executor hands its gradients to autograd: exchange them with the NCCL GradSync instead')
         net, cnet = fused.net.params, fused.cnet.params
         fused.direct_grads = (self.view_of(net), self.view_of(cnet))
         self.direct = {id(net), id(cnet)}
