@@ -253,6 +253,33 @@ int nsr_nerf_field_bwd(const nsr_nerf_t* f, const float* rays, const int32_t* ra
                        const float* xyzdir /* optional f32 [k,6]: unit-cube position + view direction per row (nsr_pack_kept); then rays,
                                               ray_indices, t_starts, t_ends are not read and every load of a tile is independent */,
                        void* stream);
+/* ---- the same two-pass field with the reference's VanillaMLP networks (NeuS learned background, configs/neus-dtu.yaml:72-105) ----
+ * f: contraction = 2 (UN_BOUNDED_SPHERE) only; L=16 F=2 grid, feature_dim 16, hidden layers 1 / 2 as above.  The networks are nn.Linear
+ * with fp32 biases, packed by the caller into the FullyFused layouts so that the kernels keep their shapes:
+ *   dmlp_h fp16 [3072] = W1 [64][32] | W2 [16][64], rows 8..15 of W2 zero;  dbias f32 [80] = b1 [64] | b2 [16], entries 8..15 zero
+ *     (feature_dim 8: feature columns 8..15 are exactly 0);
+ *   cmlp_h fp16 [7168] = W1 [64][32] | W2 [64][64] | W3 [16][64], W1 = [W[:, 0:8] | 0 (8 columns) | W[:, 8:24]] of the [64][24] layer
+ *     (features in input columns 0..15, SH4 in 16..31), rows 3..15 of W3 zero;  cbias f32 [144] = b1 [64] | b2 [64] | b3 [16].
+ *   table_h fp16: the hash table, its own buffer (not behind the density network as in nsr_nerf_*).
+ * Rounding points of the per-op path (nsr_hashgrid_fwd -> nsr_mlp_vanilla_fwd, nsr_radiance_vanilla_fwd): fp16 operands, fp32
+ * accumulation starting from the bias; the density output stays fp32 and sigma = exp(raw0 + density_bias) acts on it; the features
+ * enter the colour network rounded to fp16; rgb = sigmoid of the un-rounded fp32 colour output.
+ * nsr_bg_field_prepass / _render_fwd: as nsr_nerf_prepass / nsr_nerf_render_fwd; only rows < min(*m_dev or *k_dev, m / k) are read or
+ * written.  nsr_bg_field_bwd: as nsr_nerf_field_bwd without row_pos / xyzdir (d_sraw / d_rgb from the unchanged nsr_nerf_ray_bwd);
+ * accumulates atomically (caller zeroes) into grad_dmlp [3072], grad_table (table size), grad_dbias [80], grad_cmlp [7168] and
+ * grad_cbias [144]; the bias gradients are the column sums of the fp16 pre-activation-gradient tiles, and rows at or past the live count
+ * contribute nothing. */
+int nsr_bg_field_prepass(const nsr_nerf_t* f, const float* rays, const int32_t* ray_indices, const float* t_starts, const float* t_ends,
+                         const void* dmlp_h, const void* table_h, const float* dbias, float* alphas, int64_t m, const int64_t* m_dev,
+                         void* stream);
+int nsr_bg_field_render_fwd(const nsr_nerf_t* f, const float* rays, const int32_t* ray_indices, const float* t_starts, const float* t_ends,
+                            const float* trans, const void* dmlp_h, const void* table_h, const float* dbias, const void* cmlp_h,
+                            const float* cbias, void* enc_save_h, float* sigmas, float* rgbs, float* weights, float* acc_rgb, float* opacity,
+                            float* depth, int64_t k, const int64_t* k_dev, void* stream);
+int nsr_bg_field_bwd(const nsr_nerf_t* f, const float* rays, const int32_t* ray_indices, const float* t_starts, const float* t_ends,
+                     const void* enc_save_h, const void* dmlp_h, const float* dbias, const void* cmlp_h, const float* cbias, const float* d_sraw,
+                     const float* d_rgb, float* grad_dmlp, float* grad_table, float* grad_dbias, float* grad_cmlp, float* grad_cbias,
+                     float loss_scale, const float* amax, int64_t k, const int64_t* k_dev, void* stream);
 /* the same backward as TWO launches over the packed inputs (enc_k / d_sraw / d_rgb / xyzdir in packed row order, nsr_pack_kept):
  * (1) network half: recompute + dgrad + wgrad on tensor cores, d(encoding) -> denc_h (f16 [k,32] workspace, still multiplied by the loss
  * scale); (2) table half: a high-occupancy scatter kernel over the same rows -- runs of consecutive samples that share a cell on the

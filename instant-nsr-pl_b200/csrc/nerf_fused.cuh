@@ -28,6 +28,34 @@ __device__ __forceinline__ void nf_stage_weights(__half* smem, const __half* __r
   }
 }
 
+// network variants of the two-pass field kernels (template parameter NET): both use the smem weight layout above
+constexpr int NF_NET_FULLY_FUSED = 0;  // tcnn FullyFusedMLP (nerf-blender / nerf-colmap): bias-free, fp16 network outputs
+constexpr int NF_NET_VANILLA = 1;      // the reference's VanillaMLP (NeuS learned background): fp32 biases, fp32 network outputs
+
+// fp32 biases of the VanillaMLP variant in smem (floats): density b1 [64] | b2 [16] | colour b1 [64] | b2 [64] | b3 [16]
+// (the density and colour vectors are the nsr_bg_field_* dbias [80] and cbias [144]; outputs padded to 16 with zero biases)
+constexpr int NF_B_D1 = 0, NF_B_D2 = 64, NF_B_C1 = 80, NF_B_C2 = 144, NF_B_C3 = 208, NF_B_TOTAL = 224;
+
+__device__ __forceinline__ void nf_stage_bias(float* bias_sm, const float* __restrict__ dbias, const float* __restrict__ cbias, bool with_color) {
+  for (int i = threadIdx.x; i < (with_color ? NF_B_TOTAL : NF_B_C1); i += blockDim.x) bias_sm[i] = i < NF_B_C1 ? dbias[i] : cbias[i - NF_B_C1];
+}
+
+// accumulators of MT 16-row tiles start from zero (FullyFused) or from the fp32 bias of their column (VanillaMLP)
+template <int NET, int MT, int NT>
+__device__ __forceinline__ void nf_init_acc(float (&acc)[MT][NT][4], const float* bias_sm) {
+  if (NET == NF_NET_VANILLA) {
+    const int c2 = (threadIdx.x & 3) * 2;
+#pragma unroll
+    for (int n = 0; n < NT; ++n) {
+      const float b0 = bias_sm[n * 8 + c2], b1 = bias_sm[n * 8 + c2 + 1];
+#pragma unroll
+      for (int m = 0; m < MT; ++m) acc[m][n][0] = b0, acc[m][n][1] = b1, acc[m][n][2] = b0, acc[m][n][3] = b1;
+    }
+  } else {
+    nsr_zero_acc(acc);
+  }
+}
+
 // contraction codes of nsr_nerf_t::contraction (nerfacc.ContractionType)
 constexpr int NF_AABB = 0;
 constexpr int NF_UNBOUNDED_SPHERE = 2;

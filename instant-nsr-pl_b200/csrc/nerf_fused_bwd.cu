@@ -36,6 +36,7 @@ constexpr int T_TOTAL = T_X0B + kRows * NF_LD32;
 // packed mode: per-row inputs of two tiles in flight (floats): xyz+dir [64][6], d_sraw [64], d_rgb [64][3]
 constexpr int S_XYZ = 0, S_DS = S_XYZ + kRows * 6, S_DRGB = S_DS + kRows, S_ROWF = S_DRGB + kRows * 3;  // 640 floats per buffer
 constexpr size_t kSmemBytes = (size_t)(NF_W_TOTAL + T_TOTAL) * sizeof(__half) + 2 * S_ROWF * sizeof(float);
+constexpr size_t kSmemBytesVanilla = kSmemBytes + NF_B_TOTAL * sizeof(float);  // + the fp32 biases
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
@@ -88,7 +89,11 @@ __device__ __forceinline__ void relu_mask_pack(const float (&acc)[1][8][4], cons
 // 37 % of the stall samples were long-scoreboard waits on the row_pos -> enc / ray_indices -> rays chains and on the tile's loads).
 // The split backward (d(encoding) to memory, REDs in a separate kernel) uses nerf_bwd_net_kernel below instead.
 // CT: the field's contraction (NF_AABB / NF_UNBOUNDED_SPHERE) of the positions recomputed from the rays (!PACKED; xyzdir is AABB-only)
-template <bool PACKED, int CT>
+// NET: the network variant.  VanillaMLP (!PACKED, contracted): the recompute starts each layer from its fp32 bias and applies the colour
+// sigmoid to the un-rounded fp32 output; the table gradient goes to grad_table_sep (the table is not behind the density network there),
+// and the bias gradients are the column sums of the five pre-activation-gradient tiles (rows past the live count hold zeros in all of
+// them), one atomicAdd per bias per CTA into grad_dbias [80] / grad_cbias [144].
+template <bool PACKED, int CT, int NET>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __grid_constant__ nsr_nerf_t P, const float* __restrict__ rays,
                                                                const int32_t* __restrict__ ray_indices, const float* __restrict__ t_starts,
                                                                const float* __restrict__ t_ends, const __half* __restrict__ enc_save,
@@ -96,11 +101,16 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
                                                                const float* __restrict__ d_sraw, const float* __restrict__ d_rgb,
                                                                float* __restrict__ grad_dparams, float* __restrict__ grad_cparams,
                                                                float loss_scale, const float* __restrict__ amax_ptr, int64_t n_cap, const int64_t* __restrict__ n_dev,
-                                                               const int64_t* __restrict__ row_pos, const float* __restrict__ xyzdir) {
+                                                               const int64_t* __restrict__ row_pos, const float* __restrict__ xyzdir,
+                                                               const float* __restrict__ dbias, const float* __restrict__ cbias,
+                                                               float* __restrict__ grad_table_sep, float* __restrict__ grad_dbias,
+                                                               float* __restrict__ grad_cbias) {
   const int64_t n = n_dev ? min(*n_dev, n_cap) : n_cap;
   extern __shared__ __align__(16) __half smem[];
   __half* T = smem + NF_W_TOTAL;
   float* rowf = reinterpret_cast<float*>(smem + NF_W_TOTAL + T_TOTAL);  // [2][S_ROWF]
+  float* bias_sm = rowf + 2 * S_ROWF;                                    // VanillaMLP only
+  float bsum[2] = {0.f, 0.f};   // VanillaMLP: this thread's bias columns (threadIdx.x, threadIdx.x + 128) summed over all tiles
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
   const int r0 = warp * 16;
   if (loss_scale <= 0.f) {  // automatic: bring the largest incoming gradient to ~2^8
@@ -109,7 +119,8 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
   }
   const float inv_scale = 1.f / loss_scale;
   nf_stage_weights(smem, dparams, cparams, true);
-  float* grad_table = grad_dparams + NF_DENSITY_PARAMS;
+  if (NET == NF_NET_VANILLA) nf_stage_bias(bias_sm, dbias, cbias, true);
+  float* grad_table = NET == NF_NET_VANILLA ? grad_table_sep : grad_dparams + NF_DENSITY_PARAMS;
 
   float wacc[kSlots][2][4];
 #pragma unroll
@@ -195,11 +206,11 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
     {
       uint32_t a_in[1][2][4];
       nsr_load_afrag<1, 2>(a_in, X0, NF_LD32, r0);
-      nsr_zero_acc(acc);
+      nf_init_acc<NET>(acc, bias_sm + NF_B_D1);
       nsr_gemm_w<1, 2, 8>(acc, a_in, smem + NF_OFF_DW1, NF_LD32);
       nsr_acc_to_afrag<1, 8>(acc, a_h1, NSR_ACT_RELU);
       nsr_store_afrag<1, 4>(a_h1, T + T_H1, NSR_LD64, r0);
-      nsr_zero_acc(acc16);
+      nf_init_acc<NET>(acc16, bias_sm + NF_B_D2);
       nsr_gemm_w<1, 4, 2>(acc16, a_h1, smem + NF_OFF_DW2, NSR_LD64);
       nsr_acc_to_afrag<1, 2>(acc16, a_o, NSR_ACT_NONE);
       nsr_store_afrag<1, 1>(a_o, T + T_CI, NF_LD32, r0, 0);
@@ -212,18 +223,18 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
         a_c[0][0][j] = a_o[0][0][j];
         a_c[0][1][j] = a_sh[0][0][j];
       }
-      nsr_zero_acc(acc);
+      nf_init_acc<NET>(acc, bias_sm + NF_B_C1);
       nsr_gemm_w<1, 2, 8>(acc, a_c, smem + NF_OFF_CW1, NF_LD32);
       nsr_acc_to_afrag<1, 8>(acc, a_g1, NSR_ACT_RELU);
       nsr_store_afrag<1, 4>(a_g1, T + T_G1, NSR_LD64, r0);
-      nsr_zero_acc(acc);
+      nf_init_acc<NET>(acc, bias_sm + NF_B_C2);
       nsr_gemm_w<1, 4, 8>(acc, a_g1, smem + NF_OFF_CW2, NSR_LD64);
       nsr_acc_to_afrag<1, 8>(acc, a_g2, NSR_ACT_RELU);
       nsr_store_afrag<1, 4>(a_g2, T + T_G2, NSR_LD64, r0);
-      nsr_zero_acc(acc16);
+      nf_init_acc<NET>(acc16, bias_sm + NF_B_C3);
       nsr_gemm_w<1, 4, 2>(acc16, a_g2, smem + NF_OFF_CW3, NSR_LD64);
     }
-    // ---- d(rgb pre-activation) = d_rgb * s (1 - s), s = sigmoid(fp16(raw)); columns 0..2 only
+    // ---- d(rgb pre-activation) = d_rgb * s (1 - s), s = sigmoid(fp16(raw)) (VanillaMLP: sigmoid(raw)); columns 0..2 only
     uint32_t a_dc3[1][1][4];
     {
       float dp[4] = {0.f, 0.f, 0.f, 0.f};  // (row g: col c*2, c*2+1), (row g+8: col c*2, c*2+1)
@@ -236,7 +247,7 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
             for (int e = 0; e < 2; ++e) {
               const int col = c * 2 + e;
               if (col < 3) {
-                const float raw = __half2float(__float2half_rn(acc16[0][0][hh * 2 + e]));
+                const float raw = NET == NF_NET_VANILLA ? acc16[0][0][hh * 2 + e] : __half2float(__float2half_rn(acc16[0][0][hh * 2 + e]));
                 const float s = 1.f / (1.f + expf(-raw));
                 const float dr = PACKED ? rf[S_DRGB + (r0 + g + hh * 8) * 3 + col] : d_rgb[pi * 3 + col];
                 dp[hh * 2 + e] = dr * s * (1.f - s) * loss_scale;
@@ -357,6 +368,28 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
       const WgradTile w = wgrad_tile(warp + s * kWarps);
       const int xo = (w.x_off == T_X0) ? x0_off : w.x_off;  // the encoded features live in the current double buffer
       nsr_wgrad_tile(wacc[s][0], wacc[s][1], T + w.dy_off, w.ldy, w.m0, T + xo, w.ldx, w.n0, kRows);
+    }
+    if (NET == NF_NET_VANILLA) {  // bias gradients: column j of [dH1 (64) | dO (16) | dG1 (64) | dG2 (64) | dC3 (16)] over the tile's rows
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const int j = threadIdx.x + q * kThreads;
+        if (j < NF_B_TOTAL) {
+          const __half* col = j < NF_B_D2 ? T + T_DH1 + j : j < NF_B_C1 ? T + T_DO + (j - NF_B_D2) : j < NF_B_C2 ? T + T_DG1 + (j - NF_B_C1)
+                                                                                      : j < NF_B_C3 ? T + T_DG2 + (j - NF_B_C2) : T + T_DC3 + (j - NF_B_C3);
+          const int ld = (j >= NF_B_D2 && j < NF_B_C1) || j >= NF_B_C3 ? 24 : NSR_LD64;
+          float sum = 0.f;
+#pragma unroll 8
+          for (int r = 0; r < kRows; ++r) sum += __half2float(col[r * ld]);
+          bsum[q] += sum;
+        }
+      }
+    }
+  }
+  if (NET == NF_NET_VANILLA) {
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int j = threadIdx.x + q * kThreads;
+      if (j < NF_B_TOTAL && bsum[q] != 0.f) atomicAdd(j < NF_B_C1 ? grad_dbias + j : grad_cbias + (j - NF_B_C1), bsum[q] * inv_scale);
     }
   }
 #pragma unroll
@@ -772,10 +805,12 @@ int field_bwd_launch(const nsr_nerf_t* f, const float* rays, const int32_t* ray_
               "%s: contraction type %d not implemented here (AABB=0; UN_BOUNDED_SPHERE=2 only without xyzdir)", who, f->contraction);
   static thread_local bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(nerf_bwd_kernel<false, NF_AABB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(nerf_bwd_kernel<true, NF_AABB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(nerf_bwd_kernel<false, NF_AABB, NF_NET_FULLY_FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(nerf_bwd_kernel<false, NF_UNBOUNDED_SPHERE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+      e = cudaFuncSetAttribute(nerf_bwd_kernel<true, NF_AABB, NF_NET_FULLY_FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(nerf_bwd_kernel<false, NF_UNBOUNDED_SPHERE, NF_NET_FULLY_FUSED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)kSmemBytes);
     if (e != cudaSuccess) {
       nsr_set_error("%s: cannot reserve %zu B shared memory: %s", who, kSmemBytes, cudaGetErrorString(e));
       return 2;
@@ -787,14 +822,49 @@ int field_bwd_launch(const nsr_nerf_t* f, const float* rays, const int32_t* ray_
   if (k_dev != nullptr) grid = nsr_sm_count() * kCtasPerSm;
 #define NSR_BWD_ARGS                                                                                                                        \
   *f, rays, ray_indices, t_starts, t_ends, (const __half*)enc_save_h, (const __half*)dparams_h, (const __half*)cparams_h, d_sraw, d_rgb,    \
-      grad_dparams, grad_cparams, loss_scale, amax, k, k_dev, row_pos, xyzdir
+      grad_dparams, grad_cparams, loss_scale, amax, k, k_dev, row_pos, xyzdir, nullptr, nullptr, nullptr, nullptr, nullptr
   if (xyzdir != nullptr)
-    nerf_bwd_kernel<true, NF_AABB><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
+    nerf_bwd_kernel<true, NF_AABB, NF_NET_FULLY_FUSED><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
   else if (f->contraction == NF_UNBOUNDED_SPHERE)
-    nerf_bwd_kernel<false, NF_UNBOUNDED_SPHERE><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
+    nerf_bwd_kernel<false, NF_UNBOUNDED_SPHERE, NF_NET_FULLY_FUSED><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
   else
-    nerf_bwd_kernel<false, NF_AABB><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
+    nerf_bwd_kernel<false, NF_AABB, NF_NET_FULLY_FUSED><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(NSR_BWD_ARGS);
 #undef NSR_BWD_ARGS
+  NSR_CHECK_LAUNCH(who);
+  return 0;
+}
+
+// the VanillaMLP field (NeuS learned background): contracted, positions recomputed from the rays
+int bg_field_bwd_launch(const nsr_nerf_t* f, const float* rays, const int32_t* ray_indices, const float* t_starts, const float* t_ends,
+                        const void* enc_save_h, const void* dmlp_h, const float* dbias, const void* cmlp_h, const float* cbias, const float* d_sraw,
+                        const float* d_rgb, float* grad_dmlp, float* grad_table, float* grad_dbias, float* grad_cmlp, float* grad_cbias,
+                        float loss_scale, const float* amax, int64_t k, const int64_t* k_dev, void* stream, const char* who) {
+  NSR_REQUIRE(f != nullptr, "%s: field descriptor is NULL", who);
+  NSR_REQUIRE(f->grid.n_levels == 16 && f->grid.n_features == 2 && f->feature_dim == 16 && f->density_hidden == 1 && f->color_hidden == 2,
+              "%s: fused path needs L=16, F=2, feature_dim=16, hidden layers 1/2", who);
+  NSR_REQUIRE(f->contraction == NF_UNBOUNDED_SPHERE, "%s: the VanillaMLP field needs contraction = 2 (UN_BOUNDED_SPHERE), got %d", who,
+              f->contraction);
+  NSR_REQUIRE(loss_scale > 0.f || amax != nullptr, "%s: loss_scale <= 0 (automatic) needs the amax pointer", who);
+  if (k == 0) return 0;
+  NSR_REQUIRE(dbias != nullptr && cbias != nullptr && grad_dmlp != nullptr && grad_table != nullptr && grad_dbias != nullptr &&
+                  grad_cmlp != nullptr && grad_cbias != nullptr,
+              "%s: bias / gradient pointer is NULL", who);
+  auto kern = nerf_bwd_kernel<false, NF_UNBOUNDED_SPHERE, NF_NET_VANILLA>;
+  static thread_local bool attr_set = false;
+  if (!attr_set) {
+    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytesVanilla);
+    if (e != cudaSuccess) {
+      nsr_set_error("%s: cannot reserve %zu B shared memory: %s", who, kSmemBytesVanilla, cudaGetErrorString(e));
+      return 2;
+    }
+    attr_set = true;
+  }
+  const int64_t tiles = (k + kRows - 1) / kRows;
+  const int grid = k_dev != nullptr ? nsr_sm_count() * kCtasPerSm : (int)min((int64_t)nsr_sm_count() * kCtasPerSm, tiles);
+  kern<<<grid, kThreads, kSmemBytesVanilla, (cudaStream_t)stream>>>(*f, rays, ray_indices, t_starts, t_ends, (const __half*)enc_save_h,
+                                                                    (const __half*)dmlp_h, (const __half*)cmlp_h, d_sraw, d_rgb, grad_dmlp, grad_cmlp,
+                                                                    loss_scale, amax, k, k_dev, nullptr, nullptr, dbias, cbias, grad_table,
+                                                                    grad_dbias, grad_cbias);
   NSR_CHECK_LAUNCH(who);
   return 0;
 }
@@ -837,6 +907,14 @@ extern "C" int nsr_nerf_field_bwd(const nsr_nerf_t* f, const float* rays, const 
                                   void* stream) {
   return field_bwd_launch(f, rays, ray_indices, t_starts, t_ends, enc_save_h, dparams_h, cparams_h, d_sraw, d_rgb, grad_dparams, grad_cparams,
                           loss_scale, amax, k, k_dev, row_pos, xyzdir, stream, "nsr_nerf_field_bwd");
+}
+
+extern "C" int nsr_bg_field_bwd(const nsr_nerf_t* f, const float* rays, const int32_t* ray_indices, const float* t_starts, const float* t_ends,
+                                const void* enc_save_h, const void* dmlp_h, const float* dbias, const void* cmlp_h, const float* cbias,
+                                const float* d_sraw, const float* d_rgb, float* grad_dmlp, float* grad_table, float* grad_dbias, float* grad_cmlp,
+                                float* grad_cbias, float loss_scale, const float* amax, int64_t k, const int64_t* k_dev, void* stream) {
+  return bg_field_bwd_launch(f, rays, ray_indices, t_starts, t_ends, enc_save_h, dmlp_h, dbias, cmlp_h, cbias, d_sraw, d_rgb, grad_dmlp, grad_table,
+                             grad_dbias, grad_cmlp, grad_cbias, loss_scale, amax, k, k_dev, stream, "nsr_bg_field_bwd");
 }
 
 // The two halves of the split backward as separate entry points (what the Python side calls, so that each half shows up with its own

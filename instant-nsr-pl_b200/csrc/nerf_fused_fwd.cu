@@ -33,19 +33,31 @@ struct FwdArgs {
   float* depth;               // [n_rays]
   int64_t n;                  // sample count (capacity when n_dev is set)
   const int64_t* n_dev;       // optional: the count lives on the device (no host sync / graph capture)
+  const __half* table;        // hash table (fp16); FullyFused: dparams + NF_DENSITY_PARAMS
+  const float* dbias;         // VanillaMLP: density biases [80]
+  const float* cbias;         // VanillaMLP: colour biases [144]   (RENDER)
 };
+template <int NET>
+constexpr size_t fwd_smem() { return kSmemBytes + (NET == NF_NET_VANILLA ? NF_B_TOTAL * sizeof(float) : 0); }
 
 // CT: the field's contraction (NF_AABB / NF_UNBOUNDED_SPHERE), a template parameter so that the AABB build is unchanged
-template <int MODE, int CT>
-__global__ void __launch_bounds__(kThreads, 2) nerf_fwd_kernel(const __grid_constant__ nsr_nerf_t P, const FwdArgs a) {
+// NET: the network variant (NF_NET_FULLY_FUSED / NF_NET_VANILLA).  VanillaMLP: the accumulators start from the fp32 biases, the density
+// and colour outputs stay fp32 (the rounding points of nsr_mlp_vanilla_fwd / nsr_radiance_vanilla_fwd); the feature columns that feed the
+// colour network are rounded to fp16 as those kernels' inputs are.
+// (VanillaMLP render: the bias accumulators need a few registers more than 128, so that instantiation is sized for one CTA per SM)
+template <int MODE, int CT, int NET>
+__global__ void __launch_bounds__(kThreads, NET == NF_NET_VANILLA && MODE == MODE_RENDER ? 1 : 2) nerf_fwd_kernel(const __grid_constant__ nsr_nerf_t P, const FwdArgs a) {
   extern __shared__ __align__(16) __half smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
   __half* At = smem + NF_W_TOTAL + warp * kWarpHalves;
   __half* St = At + 32 * NF_LD32;
   float* s_sig = reinterpret_cast<float*>(St + 32 * 24);
   float* s_rgb = s_sig + 32;
-  const __half2* table = reinterpret_cast<const __half2*>(a.dparams + NF_DENSITY_PARAMS);
+  float* bias_sm = reinterpret_cast<float*>(smem + NF_W_TOTAL + kWarps * kWarpHalves);  // VanillaMLP only
+  // (FullyFused: the table follows the density network in dparams; deriving it here keeps that build's machine code as it was)
+  const __half2* table = reinterpret_cast<const __half2*>(NET == NF_NET_VANILLA ? a.table : a.dparams + NF_DENSITY_PARAMS);
   nf_stage_weights(smem, a.dparams, a.cparams, MODE == MODE_RENDER);
+  if (NET == NF_NET_VANILLA) nf_stage_bias(bias_sm, a.dbias, a.cbias, MODE == MODE_RENDER);
   __syncthreads();
 
   const int64_t n_total = a.n_dev ? min(*a.n_dev, a.n) : a.n;
@@ -98,16 +110,23 @@ __global__ void __launch_bounds__(kThreads, 2) nerf_fwd_kernel(const __grid_cons
       uint32_t a_in[2][2][4];
       nsr_load_afrag<2, 2>(a_in, At, NF_LD32, 0);
       float acc[2][8][4];
-      nsr_zero_acc(acc);
+      nf_init_acc<NET>(acc, bias_sm + NF_B_D1);
       nsr_gemm_w<2, 2, 8>(acc, a_in, smem + NF_OFF_DW1, NF_LD32);
       uint32_t a_h[2][4][4];
       nsr_acc_to_afrag<2, 8>(acc, a_h, NSR_ACT_RELU);
       float acco[2][2][4];
-      nsr_zero_acc(acco);
+      nf_init_acc<NET>(acco, bias_sm + NF_B_D2);
       nsr_gemm_w<2, 4, 2>(acco, a_h, smem + NF_OFF_DW2, NSR_LD64);
-      nsr_acc_to_afrag<2, 2>(acco, a_o, NSR_ACT_NONE);  // fp16 like tcnn's network output
+      nsr_acc_to_afrag<2, 2>(acco, a_o, NSR_ACT_NONE);  // fp16 like tcnn's network output (VanillaMLP: the colour network's input)
+      if (NET == NF_NET_VANILLA && c == 0) {  // VanillaMLP: the density output stays fp32
+#pragma unroll
+        for (int m = 0; m < 2; ++m) {
+          s_sig[m * 16 + g] = acco[m][0][0];
+          s_sig[m * 16 + g + 8] = acco[m][0][2];
+        }
+      }
     }
-    if (c == 0) {
+    if (NET != NF_NET_VANILLA && c == 0) {
 #pragma unroll
       for (int m = 0; m < 2; ++m) {
         s_sig[m * 16 + g] = nf_half_lo(a_o[m][0][0]);
@@ -129,19 +148,30 @@ __global__ void __launch_bounds__(kThreads, 2) nerf_fwd_kernel(const __grid_cons
           }
       }
       float acc[2][8][4];
-      nsr_zero_acc(acc);
+      nf_init_acc<NET>(acc, bias_sm + NF_B_C1);
       nsr_gemm_w<2, 2, 8>(acc, a_c, smem + NF_OFF_CW1, NF_LD32);
       uint32_t a_h[2][4][4];
       nsr_acc_to_afrag<2, 8>(acc, a_h, NSR_ACT_RELU);
-      nsr_zero_acc(acc);
+      nf_init_acc<NET>(acc, bias_sm + NF_B_C2);
       nsr_gemm_w<2, 4, 8>(acc, a_h, smem + NF_OFF_CW2, NSR_LD64);
       nsr_acc_to_afrag<2, 8>(acc, a_h, NSR_ACT_RELU);
       float acco[2][2][4];
-      nsr_zero_acc(acco);
+      nf_init_acc<NET>(acco, bias_sm + NF_B_C3);
       nsr_gemm_w<2, 4, 2>(acco, a_h, smem + NF_OFF_CW3, NSR_LD64);
+      if (NET == NF_NET_VANILLA && c < 2) {  // VanillaMLP: fp32 colour output, the sigmoid acts on the un-rounded value
+#pragma unroll
+        for (int m = 0; m < 2; ++m) {
+          float* r0 = s_rgb + (m * 16 + g) * 4 + c * 2;
+          float* r1 = s_rgb + (m * 16 + g + 8) * 4 + c * 2;
+          r0[0] = acco[m][0][0];
+          r0[1] = acco[m][0][1];
+          r1[0] = acco[m][0][2];
+          r1[1] = acco[m][0][3];
+        }
+      }
       uint32_t a_r[2][1][4];
       nsr_acc_to_afrag<2, 2>(acco, a_r, NSR_ACT_NONE);
-      if (c < 2) {
+      if (NET != NF_NET_VANILLA && c < 2) {
 #pragma unroll
         for (int m = 0; m < 2; ++m) {
           float* r0 = s_rgb + (m * 16 + g) * 4 + c * 2;
@@ -283,13 +313,13 @@ int check_nerf(const nsr_nerf_t* f, const char* name) {
   return 0;
 }
 
-template <int MODE, int CT>
+template <int MODE, int CT, int NET = NF_NET_FULLY_FUSED>
 int launch_fwd_ct(const nsr_nerf_t* f, const FwdArgs& a, cudaStream_t st, const char* name) {
   static thread_local bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(nerf_fwd_kernel<MODE, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(nerf_fwd_kernel<MODE, CT, NET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<NET>());
     if (e != cudaSuccess) {
-      nsr_set_error("%s: cannot reserve %zu B shared memory: %s", name, kSmemBytes, cudaGetErrorString(e));
+      nsr_set_error("%s: cannot reserve %zu B shared memory: %s", name, fwd_smem<NET>(), cudaGetErrorString(e));
       return 2;
     }
     attr_set = true;
@@ -298,7 +328,7 @@ int launch_fwd_ct(const nsr_nerf_t* f, const FwdArgs& a, cudaStream_t st, const 
   int grid = (int)min((int64_t)nsr_sm_count() * 2, (tiles + kWarps - 1) / kWarps);
   if (grid < 1) grid = 1;
   if (a.n_dev != nullptr) grid = nsr_sm_count() * 2;  // count unknown on the host: full persistent grid
-  nerf_fwd_kernel<MODE, CT><<<grid, kThreads, kSmemBytes, st>>>(*f, a);
+  nerf_fwd_kernel<MODE, CT, NET><<<grid, kThreads, fwd_smem<NET>(), st>>>(*f, a);
   NSR_CHECK_LAUNCH(name);
   return 0;
 }
@@ -311,6 +341,18 @@ int launch_fwd(const nsr_nerf_t* f, const FwdArgs& a, cudaStream_t st, const cha
   return launch_fwd_ct<MODE, NF_AABB>(f, a, st, name);
 }
 
+// the VanillaMLP field (NeuS learned background): contracted only
+template <int MODE>
+int launch_bg(const nsr_nerf_t* f, const FwdArgs& a, cudaStream_t st, const char* name) {
+  if (int e = check_nerf(f, name)) return e;
+  NSR_REQUIRE(f->contraction == NF_UNBOUNDED_SPHERE, "%s: the VanillaMLP field needs contraction = 2 (UN_BOUNDED_SPHERE), got %d", name,
+              f->contraction);
+  if (a.n == 0) return 0;
+  NSR_REQUIRE(a.dparams != nullptr && a.table != nullptr && a.dbias != nullptr && (MODE != MODE_RENDER || (a.cparams != nullptr && a.cbias != nullptr)),
+              "%s: weights / table / biases are NULL", name);
+  return launch_fwd_ct<MODE, NF_UNBOUNDED_SPHERE, NF_NET_VANILLA>(f, a, st, name);
+}
+
 }  // namespace
 
 extern "C" int nsr_nerf_density(const nsr_nerf_t* f, const float* positions, const void* dparams_h, float* density, int64_t n,
@@ -318,6 +360,7 @@ extern "C" int nsr_nerf_density(const nsr_nerf_t* f, const float* positions, con
   FwdArgs a = {};
   a.positions = positions;
   a.dparams = (const __half*)dparams_h;
+  a.table = a.dparams + NF_DENSITY_PARAMS;
   a.out0 = density;
   a.n = n;
   return launch_fwd<MODE_DENSITY>(f, a, (cudaStream_t)stream, "nsr_nerf_density");
@@ -332,6 +375,7 @@ extern "C" int nsr_nerf_prepass(const nsr_nerf_t* f, const float* rays, const in
   a.t_starts = t_starts;
   a.t_ends = t_ends;
   a.dparams = (const __half*)dparams_h;
+  a.table = a.dparams + NF_DENSITY_PARAMS;
   a.out0 = alphas;
   a.n = m;
   return launch_fwd<MODE_PREPASS>(f, a, (cudaStream_t)stream, "nsr_nerf_prepass");
@@ -349,6 +393,7 @@ extern "C" int nsr_nerf_render_fwd(const nsr_nerf_t* f, const float* rays, const
   a.t_ends = t_ends;
   a.trans = trans;
   a.dparams = (const __half*)dparams_h;
+  a.table = a.dparams + NF_DENSITY_PARAMS;
   a.cparams = (const __half*)cparams_h;
   a.enc_save = (__half*)enc_save_h;
   a.out0 = sigmas;
@@ -359,6 +404,50 @@ extern "C" int nsr_nerf_render_fwd(const nsr_nerf_t* f, const float* rays, const
   a.depth = depth;
   a.n = k;
   return launch_fwd<MODE_RENDER>(f, a, (cudaStream_t)stream, "nsr_nerf_render_fwd");
+}
+
+extern "C" int nsr_bg_field_prepass(const nsr_nerf_t* f, const float* rays, const int32_t* ray_indices, const float* t_starts,
+                                    const float* t_ends, const void* dmlp_h, const void* table_h, const float* dbias, float* alphas, int64_t m,
+                                    const int64_t* m_dev, void* stream) {
+  FwdArgs a = {};
+  a.n_dev = m_dev;
+  a.rays = rays;
+  a.ray_indices = ray_indices;
+  a.t_starts = t_starts;
+  a.t_ends = t_ends;
+  a.dparams = (const __half*)dmlp_h;
+  a.table = (const __half*)table_h;
+  a.dbias = dbias;
+  a.out0 = alphas;
+  a.n = m;
+  return launch_bg<MODE_PREPASS>(f, a, (cudaStream_t)stream, "nsr_bg_field_prepass");
+}
+
+extern "C" int nsr_bg_field_render_fwd(const nsr_nerf_t* f, const float* rays, const int32_t* ray_indices, const float* t_starts,
+                                       const float* t_ends, const float* trans, const void* dmlp_h, const void* table_h, const float* dbias,
+                                       const void* cmlp_h, const float* cbias, void* enc_save_h, float* sigmas, float* rgbs, float* weights,
+                                       float* acc_rgb, float* opacity, float* depth, int64_t k, const int64_t* k_dev, void* stream) {
+  FwdArgs a = {};
+  a.n_dev = k_dev;
+  a.rays = rays;
+  a.ray_indices = ray_indices;
+  a.t_starts = t_starts;
+  a.t_ends = t_ends;
+  a.trans = trans;
+  a.dparams = (const __half*)dmlp_h;
+  a.table = (const __half*)table_h;
+  a.dbias = dbias;
+  a.cparams = (const __half*)cmlp_h;
+  a.cbias = cbias;
+  a.enc_save = (__half*)enc_save_h;
+  a.out0 = sigmas;
+  a.rgbs = rgbs;
+  a.weights = weights;
+  a.acc_rgb = acc_rgb;
+  a.opacity = opacity;
+  a.depth = depth;
+  a.n = k;
+  return launch_bg<MODE_RENDER>(f, a, (cudaStream_t)stream, "nsr_bg_field_render_fwd");
 }
 
 extern "C" int nsr_compact_prefix(const int64_t* offsets_m, const int64_t* offsets_k, const int32_t* ray_indices_m,

@@ -17,7 +17,7 @@ import torch
 
 from . import ops
 from .lib import lib, ptr, stream, check_cuda, contig, NerfT
-from .nerfacc import ContractionType
+from .nerfacc import ContractionType, ray_aabb_intersect
 
 # Level groups of the split backward's table scatter, one launch each (top levels first).  Each group's slice of the fp32 table gradient
 # (16.5-16.8 MB here) is zeroed right in front of its launch and stays in the H100's 50 MB L2 while the REDs land on it; the whole
@@ -26,11 +26,14 @@ SCATTER_LEVEL_GROUPS = ((12, 16), (8, 12), (0, 8))
 
 
 class _NerfRender(torch.autograd.Function):
-    """(dparams, cparams) -> per-ray sums + per-sample weights; everything else rides along non-differentiably."""
+    """params -> per-ray sums + per-sample weights; everything else rides along non-differentiably.  The field's own pieces (the
+    device buffers its kernels read, the render forward and the field backward launches) come from the executor: NerfFused (params =
+    the two tcnn flat vectors) or NerfBackgroundFused (the hash table and the packed VanillaMLP weights and biases)."""
 
     @staticmethod
-    def forward(ctx, dparams, cparams, fused, rays, jitter, static=False):
-        st = fused.trace(rays, jitter, static)
+    def forward(ctx, fused, rays, jitter, static, *params):
+        kp = fused.kernel_params(*params)
+        st = fused.trace(rays, jitter, static, kp)
         n_rays, cap = rays.shape[0], st['cap']
         dev = rays.device
         acc_rgb = torch.zeros(n_rays, 3, device=dev)
@@ -39,15 +42,13 @@ class _NerfRender(torch.autograd.Function):
         sig = torch.empty(cap, device=dev)
         rgbs = torch.empty(cap, 3, device=dev)
         weights = torch.empty(cap, device=dev)
-        need_grad = dparams.requires_grad or cparams.requires_grad
+        need_grad = any(p.requires_grad for p in params)
         enc = torch.empty(cap, 32, dtype=torch.float16, device=dev) if need_grad else None
-        dh, ch = fused.dparams_half(), fused.cparams_half()
         k_dev = st['offsets_k'][n_rays:]
-        lib.call('nsr_nerf_render_fwd', fused.ref(), ptr(rays), ptr(st['ri']), ptr(st['ts']), ptr(st['te']), ptr(st['trans']), ptr(dh),
-                 ptr(ch), ptr(enc), ptr(sig), ptr(rgbs), ptr(weights), ptr(acc_rgb), ptr(opacity), ptr(depth), cap, ptr(k_dev), stream())
-        ctx.fused, ctx.n_rays, ctx.cap = fused, n_rays, cap
+        fused.render_fwd(kp, rays, st['ri'], st['ts'], st['te'], st['trans'], enc, sig, rgbs, weights, acc_rgb, opacity, depth, cap, k_dev)
+        ctx.fused, ctx.n_rays, ctx.cap, ctx.n_kp = fused, n_rays, cap, len(kp)
         ctx.set_materialize_grads(False)
-        ctx.save_for_backward(rays, st['ri'], st['ts'], st['te'], st['trans'], st['offsets_k'], enc, sig, rgbs, weights, dh, ch)
+        ctx.save_for_backward(rays, st['ri'], st['ts'], st['te'], st['trans'], st['offsets_k'], enc, sig, rgbs, weights, *kp)
         counts = torch.cat([st['offsets_m'][n_rays:], k_dev])  # [M, K] on the device
         ctx.mark_non_differentiable(st['ri'], st['ts'], st['te'], counts, *([st['overflow']] if st['overflow'] is not None else []))
         return acc_rgb, opacity, depth, weights, st['ri'], st['ts'], st['te'], counts, st['overflow']
@@ -55,11 +56,10 @@ class _NerfRender(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_rgb, g_op, g_depth, g_w, *_):
         fused = ctx.fused
-        rays, ri, ts, te, trans, offsets_k, enc, sig, rgbs, weights, dh, ch = ctx.saved_tensors
+        rays, ri, ts, te, trans, offsets_k, enc, sig, rgbs, weights, *kp = ctx.saved_tensors
         dev = rays.device
         n_rays, cap = ctx.n_rays, ctx.cap
-        gd = torch.zeros(fused.n_dparams, device=dev)
-        gc = torch.zeros(fused.n_cparams, device=dev)
+        grads = fused.zero_grads(dev)
         if cap > 0 and enc is not None:
             d_sraw = torch.empty(cap, device=dev)
             d_rgb = torch.empty(cap, 3, device=dev)
@@ -67,9 +67,8 @@ class _NerfRender(torch.autograd.Function):
             f32 = lambda t: None if t is None else contig(t, torch.float32)
             lib.call('nsr_nerf_ray_bwd', ptr(offsets_k), ptr(ts), ptr(te), ptr(trans), ptr(weights), ptr(sig), ptr(rgbs), ptr(f32(g_rgb)),
                      ptr(f32(g_op)), ptr(f32(g_depth)), ptr(f32(g_w)), ptr(d_sraw), ptr(d_rgb), ptr(amax), n_rays, stream())
-            lib.call('nsr_nerf_field_bwd', fused.ref(), ptr(rays), ptr(ri), ptr(ts), ptr(te), ptr(enc), ptr(dh), ptr(ch), ptr(d_sraw),
-                     ptr(d_rgb), ptr(gd), ptr(gc), float(fused.loss_scale), ptr(amax), cap, ptr(offsets_k[n_rays:]), None, None, stream())
-        return gd, gc, None, None, None, None
+            fused.field_bwd(kp, grads, rays, ri, ts, te, enc, d_sraw, d_rgb, amax, cap, offsets_k[n_rays:])
+        return (None, None, None, None) + tuple(grads)
 
 
 class _NerfRenderRays(torch.autograd.Function):
@@ -317,6 +316,36 @@ class NerfFused:
     def cparams_half(self):
         return self.cnet._params_half()
 
+    # ---- the field-specific pieces of the two-pass pipeline (trace / _NerfRender); NerfBackgroundFused overrides them
+    def occupancy_grid(self):
+        return self.model.occupancy_grid
+
+    def ray_t_min(self, rays):
+        """per-ray start of the march interval (None: the near plane alone)"""
+        return None
+
+    def params(self):
+        """the differentiable inputs of _NerfRender"""
+        return self.net.params, self.cnet.params
+
+    def kernel_params(self, dparams, cparams):
+        """device buffers the field kernels read, derived from params(): the fp16 copies of the two flat vectors"""
+        return self.dparams_half(), self.cparams_half()
+
+    def prepass(self, kp, rays, ri, ts, te, alphas, cap, m_dev):
+        lib.call('nsr_nerf_prepass', self.ref(), ptr(rays), ptr(ri), ptr(ts), ptr(te), ptr(kp[0]), ptr(alphas), cap, ptr(m_dev), stream())
+
+    def render_fwd(self, kp, rays, ri, ts, te, trans, enc, sig, rgbs, weights, acc_rgb, opacity, depth, cap, k_dev):
+        lib.call('nsr_nerf_render_fwd', self.ref(), ptr(rays), ptr(ri), ptr(ts), ptr(te), ptr(trans), ptr(kp[0]), ptr(kp[1]), ptr(enc),
+                 ptr(sig), ptr(rgbs), ptr(weights), ptr(acc_rgb), ptr(opacity), ptr(depth), cap, ptr(k_dev), stream())
+
+    def zero_grads(self, dev):
+        return [torch.zeros(self.n_dparams, device=dev), torch.zeros(self.n_cparams, device=dev)]
+
+    def field_bwd(self, kp, grads, rays, ri, ts, te, enc, d_sraw, d_rgb, amax, cap, k_dev):
+        lib.call('nsr_nerf_field_bwd', self.ref(), ptr(rays), ptr(ri), ptr(ts), ptr(te), ptr(enc), ptr(kp[0]), ptr(kp[1]), ptr(d_sraw),
+                 ptr(d_rgb), ptr(grads[0]), ptr(grads[1]), float(self.loss_scale), ptr(amax), cap, ptr(k_dev), None, None, stream())
+
     @torch.no_grad()
     def density(self, positions):
         """density at world positions (occ_eval_fn, models/nerf.py:49-52)."""
@@ -327,13 +356,15 @@ class NerfFused:
         return out.reshape(positions.shape[:-1])
 
     @torch.no_grad()
-    def trace(self, rays, jitter=None, static=True):
+    def trace(self, rays, jitter=None, static=True, kp=None):
         """march + sigma_fn visibility pre-pass + compaction: the ``with torch.no_grad(): ray_marching(...)`` block of
         models/nerf.py:82-93, without a host sync.  Buffers have capacity n_rays * cap_per_ray; the true counts
         are offsets_m[n_rays] (marched) and offsets_k[n_rays] (kept) on the device.  Contracted: the cone marcher, with
         capacity-length buffers when static (see static_capacity; 'overflow' flags dropped samples), else buffers of exactly
-        the marched count (one device->host read)."""
+        the marched count (one device->host read).  kp: kernel_params() (default: those of the current parameters)."""
         m = self.model
+        if kp is None:
+            kp = self.kernel_params(*self.params())
         dev = rays.device
         n = rays.shape[0]
         cap = n * self.cap_per_ray
@@ -341,7 +372,7 @@ class NerfFused:
         u = None
         if m.randomized:
             u = torch.rand(n, device=dev) if jitter is None else contig(jitter.to(dev), torch.float32)
-        grid = m.occupancy_grid
+        grid = self.occupancy_grid()
         i32 = lambda k: torch.empty(k, dtype=torch.int32, device=dev)
         f32 = lambda k: torch.empty(k, dtype=torch.float32, device=dev)
         overflow = None
@@ -349,7 +380,7 @@ class NerfFused:
             if static and self.static_capacity is not None:
                 cap = int(self.static_capacity)
             mc = ops.march_cone(self.march, rays, u, max(0.0, self.near), min(1e10, self.far), grid.bits(), self.cap_per_ray,
-                                cap=cap if static else None)
+                                t_min=self.ray_t_min(rays), cap=cap if static else None)
             ri_m, ts_m, te_m, offsets_m, overflow = mc['ray_indices'], mc['t_starts'], mc['t_ends'], mc['offsets'], mc['overflow']
             cap = ri_m.shape[0]
         else:
@@ -362,8 +393,7 @@ class NerfFused:
             ri_m, ts_m, te_m = i32(cap), f32(cap), f32(cap)
             lib.call('nsr_march_rays_expand', mref, ptr(masks), words, ptr(t_min), ptr(offsets_m), ptr(ri_m), ptr(ts_m), ptr(te_m), n, stream())
         alphas = f32(cap)
-        lib.call('nsr_nerf_prepass', self.ref(), ptr(rays), ptr(ri_m), ptr(ts_m), ptr(te_m), ptr(self.dparams_half()), ptr(alphas), cap,
-                 ptr(offsets_m[n:]), stream())
+        self.prepass(kp, rays, ri_m, ts_m, te_m, alphas, cap, offsets_m[n:])
         keep = torch.empty(cap, dtype=torch.uint8, device=dev)
         trans, kept = f32(cap), i32(n)
         lib.call('nsr_visibility', ptr(alphas), ptr(offsets_m), ptr(keep), ptr(trans), ptr(kept), self.early_stop_eps, self.alpha_thre, n, stream())
@@ -421,8 +451,7 @@ class NerfFused:
 
     def _render_two_pass(self, rays, jitter, static):
         m = self.model
-        acc_rgb, opacity, depth, weights, ri, ts, te, counts, overflow = _NerfRender.apply(self.net.params, self.cnet.params, self, rays,
-                                                                                          jitter, static)
+        acc_rgb, opacity, depth, weights, ri, ts, te, counts, overflow = _NerfRender.apply(self, rays, jitter, static, *self.params())
         comp_rgb = acc_rgb + m.background_color * (1.0 - opacity)
         out = {'comp_rgb': comp_rgb, 'opacity': opacity, 'depth': depth, 'rays_valid': opacity > 0,
                'num_samples': counts[1:].to(torch.int32)}
@@ -443,3 +472,110 @@ class NerfFused:
             out.update({'weights': w.view(-1), 'points': ((ts_ + te_) / 2.).view(-1), 'intervals': (te_ - ts_).view(-1),
                         'ray_indices': ri_.long().view(-1)})
         return out
+
+
+class NerfBackgroundFused(NerfFused):
+    """Static-shape executor of the NeuS learned background (NeuSModel.forward_bg_, models/neus.py:153-169 of the reference) on the
+    contracted two-pass pipeline of NerfFused -- cone marcher, visibility pre-pass, compaction, render forward, field backward -- with the
+    VanillaMLP variant of the field kernels (nsr_bg_field_*).  The field is the neus-dtu background: VolumeDensity HashGrid (L=16, F=2)
+    -> VanillaMLP 64 -> 8 with trunc_exp, VolumeRadiance [feature 8 | SH4] -> VanillaMLP 64 x 2 -> 3 with a sigmoid.  Each ray's interval
+    starts where it leaves the foreground box (the background near plane when it misses the box) and ends at the far plane."""
+
+    def __init__(self, model):
+        self.model = model
+        geo, tex = model.geometry_bg, model.texture_bg
+        self.enc = geo.encoding_with_network.encoding.encoding   # tcnn.Encoding: owns the hash table
+        self.dnet, self.cnet = geo.encoding_with_network.network, tex.network   # VanillaMLP
+        self.grid = self.enc.grid
+        s = NerfT()
+        s.grid = self.grid.struct
+        s.radius = float(model.config.radius)
+        s.density_bias = float(geo.config.density_bias)
+        s.feature_dim, s.density_hidden, s.color_hidden = 16, 1, 2
+        s.contraction = ContractionType.UN_BOUNDED_SPHERE.value
+        self.struct = s
+        self.contracted, self.mode = True, 'two_pass'
+        grid = model.occupancy_grid_bg
+        step, cone = model.render_step_size_bg, model.cone_angle_bg
+        self.march = ops.march_struct(grid.roi_host(), grid._res, s.contraction, step, cone)
+        # per-ray near = max(t_min[ray], 0) (nerfacc's order), far = the background far plane; no ray starts before t = 0
+        self.near, self.far = 0.0, float(model.far_plane_bg)
+        self.cap_per_ray = ops.cone_step_bound(0.0, self.far, step, cone)
+        # rows of the static sample buffers (None = n_rays * cap_per_ray, which never overflows); config static_sample_capacity_bg
+        # overrides it.  A step whose samples do not fit sets out['overflow'].
+        self.static_capacity = model.config.get('static_sample_capacity_bg', None)
+        self.loss_scale = 0.0   # chosen on the device from the incoming gradient magnitude
+        self.early_stop_eps, self.alpha_thre = 1e-4, 0.0
+        self.last_stats = {}
+
+    @staticmethod
+    def unsupported(model):
+        """None when the model's learned background is the shape the kernels implement, else what is missing (a message)."""
+        from . import tcnn
+        from .models.fields import VolumeDensity, VolumeRadiance
+        from .models.networks import EncodingWithNetwork, VanillaMLP
+        cfg = model.config
+        if not cfg.grid_prune:
+            return 'the background occupancy grid (grid_prune)'
+        geo, tex = model.geometry_bg, model.texture_bg
+        if not (isinstance(geo, VolumeDensity) and isinstance(geo.encoding_with_network, EncodingWithNetwork)):
+            return 'a volume-density background with a VanillaMLP network'
+        enc, dnet = geo.encoding_with_network.encoding, geo.encoding_with_network.network
+        if enc.include_xyz or not isinstance(enc.encoding, tcnn.Encoding) or enc.encoding.grid is None or enc.encoding.grid.n_levels != 16:
+            return 'a 16-level HashGrid background encoding (F=2) without include_xyz'
+        if not isinstance(dnet, VanillaMLP) or dnet.sphere_init or dnet.n_neurons != 64 or dnet.n_hidden_layers != 1 or geo.n_output_dims != 8:
+            return 'a background density VanillaMLP 32 -> 64 (ReLU) -> 8'
+        if (geo.config.get('density_activation') != 'trunc_exp' or 'feature_activation' in geo.config
+                or str(geo.config.mlp_network_config.get('output_activation', 'none')).lower() != 'none'):
+            return 'trunc_exp background density with a linear network output and no feature activation'
+        if not isinstance(tex, VolumeRadiance) or tex.n_dir_dims != 3 or tex.config.input_feature_dim != 8:
+            return 'a volume-radiance background texture on 8 features'
+        denc = tex.encoding
+        if denc.include_xyz or not (isinstance(denc.encoding, tcnn.Encoding) and denc.encoding.otype == 'SphericalHarmonics'
+                                    and int(denc.encoding.encoding_config.get('degree', 4)) == 4):
+            return 'a degree-4 SphericalHarmonics background direction encoding'
+        cnet = tex.network
+        if not isinstance(cnet, VanillaMLP) or cnet.sphere_init or cnet.n_neurons != 64 or cnet.n_hidden_layers != 2:
+            return 'a background colour VanillaMLP 24 -> 64 -> 64 (ReLU) -> 3'
+        out_act = str(tex.config.mlp_network_config.get('output_activation', 'none')).lower()
+        col_act = str(tex.config.get('color_activation', 'none')).lower()
+        if sorted([out_act, col_act]) != ['none', 'sigmoid']:
+            return 'a sigmoid background colour'
+        return None
+
+    def occupancy_grid(self):
+        return self.model.occupancy_grid_bg
+
+    def ray_t_min(self, rays):
+        # NeuSModel.forward_bg_: start where the ray leaves the foreground box; rays that miss it start at the background near plane
+        _, t_max = ray_aabb_intersect(rays[:, 0:3].contiguous(), rays[:, 3:6].contiguous(), self.model.scene_aabb)
+        return torch.where(t_max > 1e9, self.model.near_plane_bg, t_max)
+
+    def params(self):
+        """the hash table (fp32 master) and the packed VanillaMLP weights / biases (ops.pack_background_field; differentiable)"""
+        return (self.enc.params,) + ops.pack_background_field(self.dnet.linear_params(), self.cnet.linear_params())
+
+    def kernel_params(self, table, dmlp, dbias, cmlp, cbias):
+        return (self.enc._params_half(), dmlp.detach().to(torch.float16).contiguous(), contig(dbias.detach(), torch.float32),
+                cmlp.detach().to(torch.float16).contiguous(), contig(cbias.detach(), torch.float32))
+
+    def prepass(self, kp, rays, ri, ts, te, alphas, cap, m_dev):
+        table_h, dmlp_h, dbias = kp[:3]
+        lib.call('nsr_bg_field_prepass', self.ref(), ptr(rays), ptr(ri), ptr(ts), ptr(te), ptr(dmlp_h), ptr(table_h), ptr(dbias), ptr(alphas),
+                 cap, ptr(m_dev), stream())
+
+    def render_fwd(self, kp, rays, ri, ts, te, trans, enc, sig, rgbs, weights, acc_rgb, opacity, depth, cap, k_dev):
+        table_h, dmlp_h, dbias, cmlp_h, cbias = kp
+        lib.call('nsr_bg_field_render_fwd', self.ref(), ptr(rays), ptr(ri), ptr(ts), ptr(te), ptr(trans), ptr(dmlp_h), ptr(table_h), ptr(dbias),
+                 ptr(cmlp_h), ptr(cbias), ptr(enc), ptr(sig), ptr(rgbs), ptr(weights), ptr(acc_rgb), ptr(opacity), ptr(depth), cap, ptr(k_dev),
+                 stream())
+
+    def zero_grads(self, dev):
+        return [torch.zeros(n, device=dev) for n in (self.grid.n_params, 3072, 80, 7168, 144)]
+
+    def field_bwd(self, kp, grads, rays, ri, ts, te, enc, d_sraw, d_rgb, amax, cap, k_dev):
+        table_h, dmlp_h, dbias, cmlp_h, cbias = kp
+        g_table, g_dmlp, g_dbias, g_cmlp, g_cbias = grads
+        lib.call('nsr_bg_field_bwd', self.ref(), ptr(rays), ptr(ri), ptr(ts), ptr(te), ptr(enc), ptr(dmlp_h), ptr(dbias), ptr(cmlp_h), ptr(cbias),
+                 ptr(d_sraw), ptr(d_rgb), ptr(g_dmlp), ptr(g_table), ptr(g_dbias), ptr(g_cmlp), ptr(g_cbias), float(self.loss_scale), ptr(amax),
+                 cap, ptr(k_dev), stream())

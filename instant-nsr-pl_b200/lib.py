@@ -136,6 +136,9 @@ _SIGNATURES = {
     'nsr_nerf_field_bwd_net': [P, P, P, P, P, P, P, P, F32, P, I64, P, P, P, P],
     'nsr_nerf_table_scatter': [P, P, I32, P, F32, P, P, I64, P, I32, I32, I32, P],
     'nsr_nerf_field_bwd_tc': [P, P, P, P, P, P, P, P, F32, P, I64, P, P, P, P],
+    'nsr_bg_field_prepass': [P, P, P, P, P, P, P, P, P, I64, P, P],
+    'nsr_bg_field_render_fwd': [P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, I64, P, P],
+    'nsr_bg_field_bwd': [P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, F32, P, I64, P, P],
     'nsr_distortion_fwd': [P, P, P, P, I32, P, P, I64, P, P],
     'nsr_distortion_bwd': [P, P, P, P, I32, P, P, P, I64, P, P],
 }

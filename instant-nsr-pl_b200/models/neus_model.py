@@ -101,6 +101,7 @@ class NeuSModel(BaseModel):
         self.cos_anneal_ratio = 1.0
         self._cos_dev = None        # device copy of cos_anneal_ratio for the static (CUDA-graph) path
         self._march_static = None
+        self._bg_fused = None       # static path: the learned background on the fused field kernels (fused.NerfBackgroundFused)
 
     def _inv_s(self, n):
         return self.variance(torch.zeros([1, 3]))[:, :1].clip(1e-6, 1e6).expand(n, 1)
@@ -181,12 +182,27 @@ class NeuSModel(BaseModel):
         return self._nerf_like(rays, self.geometry_bg, self.texture_bg, self.occupancy_grid_bg if self.config.grid_prune else None,
                                near, self.far_plane_bg, self.render_step_size_bg, self.cone_angle_bg, None, jitter=jitter)
 
+    def _static_background(self):
+        """the learned background's static executor (built on the first static forward), or NotImplementedError naming what is missing"""
+        from ..fused import NerfBackgroundFused
+        if self._bg_fused is None:
+            if not (getattr(self.geometry, '_fused', False) or getattr(self.geometry, '_fused_fd', False)):
+                raise NotImplementedError('static NeuS forward with a learned background: needs the fused foreground SDF field (include_xyz '
+                                          'HashGrid + sphere-init VanillaMLP, analytic or finite-difference normals); a ProgressiveBandHashGrid '
+                                          'with analytic normals (neus-colmap) runs the per-op field')
+            missing = NerfBackgroundFused.unsupported(self)
+            if missing is not None:
+                raise NotImplementedError(f'static NeuS forward with a learned background: needs {missing}')
+            self._bg_fused = NerfBackgroundFused(self)
+        return self._bg_fused
+
     def _forward_static(self, rays, jitter=None):
         cfg = self.config
         fd = cfg.geometry.grad_type == 'finite_difference' and getattr(self.geometry, '_fused_fd', False)
-        if cfg.learned_background or not cfg.grid_prune or not (cfg.geometry.grad_type == 'analytic' or fd) or not rays.is_cuda:
-            raise NotImplementedError("static NeuS forward: foreground-only configs with grid_prune and analytic normals (neus-blender) or "
+        if not cfg.grid_prune or not (cfg.geometry.grad_type == 'analytic' or fd) or not rays.is_cuda:
+            raise NotImplementedError("static NeuS forward: configs with grid_prune and analytic normals (neus-blender, neus-dtu) or "
                                       "fused finite-difference normals (neuralangelo-dtu-wmask) on CUDA")
+        bg_fused = self._static_background() if cfg.learned_background else None
         import math
         n_rays, dev = rays.shape[0], rays.device
         cap = int(cfg.get('static_sample_capacity', 1 << 19))
@@ -222,6 +238,16 @@ class NeuSModel(BaseModel):
                'intervals': dists.view(-1), 'ray_indices': ri32, 'num_samples_dev': k_dev, 'overflow': m['overflow']}
         if fd:
             out['sdf_laplace_samples'] = sdf_laplace
+        if bg_fused is not None:
+            # capacity-length background buffers (two-pass static layout: weights / t_starts / t_ends / ray_indices, live rows
+            # num_samples_bg); its own sample overflow joins the foreground's
+            out_bg = bg_fused.render(rays, jitter, static=True)
+            out['overflow'] = out['overflow'] | out_bg.pop('overflow')
+            out.update({k + '_bg': v for k, v in out_bg.items()})
+            bg = out_bg['comp_rgb']
+            out.update({'comp_rgb_full': comp_rgb + bg * (1.0 - opacity), 'num_samples_full': num + out_bg['num_samples'],
+                        'rays_valid_full': valid | out_bg['rays_valid']})
+            return out
         bg = self.background_color[None, :].expand(*comp_rgb.shape)
         out.update({'comp_rgb_bg': bg, 'num_samples_bg': torch.zeros_like(num), 'rays_valid_bg': torch.zeros_like(valid),
                     'comp_rgb_full': comp_rgb + bg * (1.0 - opacity), 'num_samples_full': num, 'rays_valid_full': valid})

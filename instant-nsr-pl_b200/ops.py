@@ -787,6 +787,27 @@ def pack_vanilla_radiance(layers):
     return weights, bias
 
 
+def pack_background_field(density_layers, color_layers):
+    """The NeuS learned background's VanillaMLP networks (density 32 -> 64 -> 8, colour [feature 8 | SH4 16] -> 64 -> 64 -> 3) -> their
+    packed form for nsr_bg_field_* (the FullyFused shapes of the fused NeRF field): (dmlp f32 [3072], dbias [80], cmlp [7168], cbias [144]).
+    Density W2 / b2 are padded with zero rows to 16 outputs, so feature columns 8..15 are exactly 0; colour W1 [64, 24] becomes
+    [W[:, 0:8] | 0 (8 columns) | W[:, 8:24]], which puts the SH columns at 16..31 where the kernels keep them.  Plain differentiable torch
+    ops: autograd hands the kernels' flat gradients back to the layers (and through a weight-norm reparametrisation, if any)."""
+    (D1, db1), (D2, db2) = density_layers
+    (C1, cb1), (C2, cb2), (C3, cb3) = color_layers
+    if (tuple(D1.shape) != (64, 32) or tuple(D2.shape) != (8, 64) or tuple(C1.shape) != (64, 24) or tuple(C2.shape) != (64, 64)
+            or tuple(C3.shape) != (3, 64)):
+        raise NotImplementedError('fused background field: needs density 32 -> 64 -> 8 and colour 24 -> 64 -> 64 -> 3 VanillaMLP layers')
+    F = torch.nn.functional
+    D1, D2, C1, C2, C3 = (w.float() for w in (D1, D2, C1, C2, C3))
+    dmlp = torch.cat([D1.reshape(-1), F.pad(D2, (0, 0, 0, 8)).reshape(-1)])
+    dbias = torch.cat([db1.float(), F.pad(db2.float(), (0, 8))])
+    C1 = torch.cat([C1[:, :8], C1.new_zeros(64, 8), C1[:, 8:]], dim=1)
+    cmlp = torch.cat([C1.reshape(-1), C2.reshape(-1), F.pad(C3, (0, 0, 0, 13)).reshape(-1)])
+    cbias = torch.cat([cb1.float(), cb2.float(), F.pad(cb3.float(), (0, 13))])
+    return dmlp, dbias, cmlp, cbias
+
+
 def radiance_vanilla(spec, feat, dirs, extra, layers):
     """cat[feat | SH4(dirs) | extra] -> VanillaMLP (layers = [(W, b)] * 3, see pack_vanilla_radiance) -> fp32 rgb [n,3] (+ sigmoid
     when spec.act_mode != 0).  fp16 tensor-core operands with fp32 accumulation against the reference's fp32 cuBLAS GEMMs."""
