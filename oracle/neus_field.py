@@ -2,7 +2,7 @@
 models/geometry.py:158-180; encoding = CompositeEncoding[2x-1 | HashGrid] network_utils.py:68-79; network = VanillaMLP with one
 hidden layer and Softplus(beta=100), network_utils.py:95-139) -- CPU restatement of what the fused CUDA kernels compute, in
 plain torch WITHOUT autograd.  tests/test_oracle_kat.py checks it against autograd (incl. the second-order terms the eikonal
-loss needs); tests/test_gpu_neus.py checks the kernels against it.
+loss needs); tests/helpers/neus_field_ref.py restates it with per-entry error bounds for the kernel tests.
 
 Notation (per sample): e = [2 x01 - 1 (3) | hash(x01) (LF)];  z = W1 e + b1;  h = softplus_beta(z);  s = sigmoid(beta z) = dh/dz
 out = W2 h + b2 (sdf = out_0);  u = s * W2[0];  q = W1^T u;  grad_world = (2 q_xyz + J^T q_hash) / (2 r),  J = d hash / d x01.
@@ -16,12 +16,19 @@ import torch
 from . import hashgrid
 
 
-def _level_terms(x01, table, lt, l):
-    """cells / weights / derivative weights of level l: idx [N,8], w [N,8], dw [N,8,3] (d w_c / d x01, scale included)."""
+def x01_f32(points, radius):
+    """the kernels' normalised position fp32(fp32(p + r) * fp32(1 / (2 r))): exactly the value their cell rule sees"""
+    r = torch.tensor(radius, dtype=torch.float32)
+    return (points.float() + r) * (1.0 / (2.0 * r))
+
+
+def _level_terms(x01, table, lt, l, f32_frac=False):
+    """cells / weights / derivative weights of level l: idx [N,8], w [N,8], dw [N,8,3] (d w_c / d x01, scale included).
+    f32_frac: the fraction is the kernels' fp32 pos - floor(pos) (exact given pos) instead of the unrounded fp64 one."""
     scale = float(lt['scale'][l])
     pos32 = hashgrid.fma_f32(x01.float(), torch.tensor(scale, dtype=torch.float32), torch.tensor(0.5))
     cell = torch.floor(pos32)
-    frac = (x01.double() * scale + 0.5 - cell.double())
+    frac = (pos32.double() if f32_frac else x01.double() * scale + 0.5) - cell.double()
     ci = cell.to(torch.int64)
     res, size, dense, off = int(lt['res'][l]), int(lt['size'][l]), bool(lt['dense'][l]), int(lt['offset'][l])
     idx, w, dw = [], [], []
@@ -35,14 +42,16 @@ def _level_terms(x01, table, lt, l):
     return torch.stack(idx, 1), torch.stack(w, 1), torch.stack(dw, 1)
 
 
-def forward(points, table, lt, W1, b1, W2, b2, radius, beta=100.0):
-    """-> sdf [N], grad_world [N,3], feature [N,n_out], cache."""
-    x01 = (points.double() + radius) / (2 * radius)
+def forward(points, table, lt, W1, b1, W2, b2, radius, beta=100.0, kernel_cells=False):
+    """-> sdf [N], grad_world [N,3], feature [N,n_out], cache.
+    kernel_cells: take x01 and the cell fractions as the kernels compute them in fp32 (x01_f32, then fp32 pos - floor(pos)), so that
+    every level picks the same cell as the kernels, even for samples one ulp from a cell face; the rest stays fp64."""
+    x01 = x01_f32(points, radius).double() if kernel_cells else (points.double() + radius) / (2 * radius)
     tab = table.double().view(-1, 2)
     L = lt['n_levels']
     feats, J = [], []
     for l in range(L):
-        idx, w, dw = _level_terms(x01, tab, lt, l)
+        idx, w, dw = _level_terms(x01, tab, lt, l, kernel_cells)
         v = tab[idx]                                     # [N,8,2]
         feats.append((w[..., None] * v).sum(1))          # [N,2]
         J.append(torch.einsum('ncd,ncf->nfd', dw, v))    # [N,2,3]
@@ -55,7 +64,7 @@ def forward(points, table, lt, W1, b1, W2, b2, radius, beta=100.0):
     u = s * W2.double()[0]
     q = u @ W1.double()                                  # [N, 3+2L]
     g01 = 2 * q[:, :3] + torch.einsum('nfd,nf->nd', J, q[:, 3:])
-    return out[:, 0], g01 / (2 * radius), out, dict(x01=x01, e=e, J=J, z=z, h=h, s=s, u=u, q=q)
+    return out[:, 0], g01 / (2 * radius), out, dict(x01=x01, e=e, J=J, z=z, h=h, s=s, u=u, q=q, kernel_cells=kernel_cells)
 
 
 def backward(cache, table, lt, W1, b1, W2, b2, radius, g_out, g_grad, beta=100.0):
@@ -74,7 +83,7 @@ def backward(cache, table, lt, W1, b1, W2, b2, radius, g_out, g_grad, beta=100.0
     x01 = cache['x01']
     tab = table.double().view(-1, 2)
     for l in range(lt['n_levels']):
-        idx, w, dw = _level_terms(x01, tab, lt, l)
+        idx, w, dw = _level_terms(x01, tab, lt, l, cache.get('kernel_cells', False))
         ebl = eb[:, 3 + 2 * l: 5 + 2 * l]                # [N,2]
         ql = q[:, 3 + 2 * l: 5 + 2 * l]
         coef = torch.einsum('ncd,nd->nc', dw, gx)        # [N,8]

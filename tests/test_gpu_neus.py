@@ -155,49 +155,6 @@ def test_neus_dtu_learned_background_runs_and_composes():
     assert e['comp_rgb_full'].device.type == 'cpu' and 'sdf_samples' not in e and 'inv_s' in e
 
 
-def test_neus_field_kernels_match_manual_oracle():
-    """nsr_neus_field_fwd / _bwd (fused hash grid + fp32 SDF MLP + analytic normal, first AND second order backward) against
-    oracle/neus_field.py (hand derivation, itself checked against autograd in tests/test_oracle_kat.py)."""
-    from nsr_b200 import ops
-    from oracle import neus_field, hashgrid as ohash
-    D = torch.device('cuda:0')
-    cfg = dict(otype='HashGrid', n_levels=16, n_features_per_level=2, log2_hashmap_size=19, base_resolution=32,
-               per_level_scale=1.3195079107728942)
-    spec = ops.GridSpec(cfg)
-    lt = ohash.level_table(cfg)
-    g = torch.Generator().manual_seed(0)
-    n, n_out, r = 3000, 13, 1.5
-    # amplitude ~ 1/scale_l per level: every level contributes O(1) to the normal, so a sample that lands on the other side of a
-    # cell face (one-ulp position difference) perturbs the result only slightly
-    table = torch.zeros(lt['n_params'] // 2, 2)
-    for l in range(16):
-        a, b = int(lt['offset'][l]), int(lt['offset'][l + 1])
-        table[a:b] = (torch.rand(b - a, 2, generator=g) * 2 - 1) * (0.5 / float(lt['scale'][l]))
-    table = table.flatten().half().float()
-    W1 = torch.randn(64, 35, generator=g) * 0.1
-    W1[:, :3] *= 3
-    b1 = torch.randn(64, generator=g) * 0.02
-    W2 = torch.randn(n_out, 64, generator=g) * 0.2
-    b2 = torch.randn(n_out, generator=g) * 0.1
-    pts = (torch.rand(n, 3, generator=g) * 2 - 1) * 1.3
-    g_out = torch.randn(n, n_out, generator=g) * 0.01
-    g_grad = torch.randn(n, 3, generator=g) * 0.01
-    tp = table.to(D).requires_grad_(True)
-    ws = [t.to(D).requires_grad_(True) for t in (W1, b1, W2, b2)]
-    sdf, grad, feat = ops.neus_sdf(spec, r, pts.to(D), tp, tp.detach().half(), *ws)
-    ((feat * g_out.to(D)).sum() + (grad * g_grad.to(D)).sum()).backward()
-    sdf_r, grad_r, out_r, cache = neus_field.forward(pts, table, lt, W1, b1, W2, b2, r)
-    gm = neus_field.backward(cache, table, lt, W1, b1, W2, b2, r, g_out, g_grad)
-    assert (sdf.detach().cpu() - sdf_r.float()).abs().max().item() <= 1e-4
-    assert (feat.detach().cpu() - out_r.float()).abs().max().item() <= 1e-4
-    gerr = (grad.detach().cpu() - grad_r.float()).abs().max(dim=-1).values
-    assert (gerr > 1e-3 * grad_r.abs().max().item()).float().mean().item() <= 5e-3   # cell-face flips (see the model-level test)
-    for name, t in zip(('W1', 'b1', 'W2', 'b2'), ws):
-        assert cos(t.grad.cpu(), gm[name].float()) >= 0.999, name
-        assert (t.grad.cpu() - gm[name].float()).abs().max().item() <= 3e-2 * gm[name].abs().max().item(), name
-    assert cos(tp.grad.cpu(), gm['table'].float()) >= 0.995
-
-
 def test_neus_model_composed_path_still_matches_fused():
     """geometry.fused = False falls back to the per-op composition (tcnn-shaped hash grid with double backward + torch VanillaMLP)."""
     from nsr_b200 import configs, models
