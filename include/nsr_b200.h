@@ -368,6 +368,17 @@ int nsr_neus_field_bwd(const nsr_grid_t* g, const float* points, const void* tab
                        const float* b2, float radius, int32_t n_out, const float* g_out, const float* g_sdf, const float* g_grad,
                        const float* amax, float* grad_table, float* dW1, float* db1, float* dW2, float* db2, int64_t n, const int64_t* n_dev,
                        void* stream);
+/* The same field under a ProgressiveBandHashGrid level mask: hash levels >= n_active contribute 0 to the features, the analytic normal,
+ * every backward term and the table gradient, and are neither gathered nor scattered (their grad_table slices are left untouched, their
+ * dW1 columns receive 0).  n_active: device float (clamped to [0, 16], read on the device, so a captured graph follows the schedule).
+ * n_active = 16 gives exactly nsr_neus_field_fwd / _bwd.  NSR_NEUS_FWD=scalar selects the masked thread-per-sample forward. */
+int nsr_neus_field_fwd_levels(const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1, const float* W2,
+                              const float* b2, float radius, int32_t n_out, const float* n_active, float* sdf, float* grad, float* feature, int64_t n,
+                              const int64_t* n_dev, void* stream);
+int nsr_neus_field_bwd_levels(const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1, const float* W2,
+                              const float* b2, float radius, int32_t n_out, const float* n_active, const float* g_out, const float* g_sdf,
+                              const float* g_grad, const float* amax, float* grad_table, float* dW1, float* db1, float* dW2, float* db2, int64_t n,
+                              const int64_t* n_dev, void* stream);
 /* ---- fused NeuS SDF field with finite-difference normals + Laplacian (grad_type 'finite_difference': models/geometry.py:181-199) ----
  * Same field and weights as nsr_neus_field_*, evaluated at the centre x_0 = (p + r) / 2r and at the six stencil points
  * (clamp(p +- eps e_a, -r, r) + r) / 2r (true fp32 division); hash levels >= n_active contribute 0 (ProgressiveBandHashGrid mask).

@@ -72,6 +72,17 @@ def neus_dtu(radius=1.0):
     return cfg
 
 
+def neus_colmap(radius=0.6):
+    """configs/neus-colmap.yaml:15-110: neus-dtu's model (learned NeRF++ background, VanillaMLP colour networks) with a
+    ProgressiveBandHashGrid foreground (levels switched on every 1000 steps from level 4, analytic normals) and 256 background samples
+    per ray.  The fused masked field is opt-in: set geometry['fused_progressive'] = True."""
+    cfg = neus_dtu(radius)
+    cfg.update(num_samples_per_ray_bg=256)
+    cfg['geometry']['xyz_encoding_config'] = dict(_HASH_NEUS, otype='ProgressiveBandHashGrid', include_xyz=True, start_level=4, start_step=0,
+                                                  update_steps=1000)
+    return cfg
+
+
 def neuralangelo_dtu(radius=1.0):
     """configs/neuralangelo-dtu-wmask.yaml:18-75: NeuS with a ProgressiveBandHashGrid (levels switched on every 1000 steps), finite-difference
     normals with the progressive step, VanillaMLP colour network; no learned background."""

@@ -48,12 +48,25 @@ __device__ __forceinline__ float softplus100(float z, float& s) {
   return bz > 20.f ? z : log1pf(__expf(bz)) * 0.01f;  // torch.nn.Softplus(beta=100, threshold=20)
 }
 
-// gather: e[3..34] (features) and optionally qb[3..34] = J gx (directional derivative of every feature along gx)
-template <bool WITH_QB>
+// MASK: hash levels >= n_active contribute 0 (ProgressiveBandHashGrid: the level mask multiplies the features, so a masked level's
+// features, Jacobian and table gradient are all zero).  The kernels read n_active on the device (uniform per CTA), so a captured graph
+// follows the schedule; masked levels are neither gathered nor scattered.
+__device__ __forceinline__ int load_n_active(const float* __restrict__ n_active) {
+  return (int)fminf(fmaxf(__ldg(n_active), 0.f), 16.f);   // NaN -> 0
+}
+
+// gather: e[3..34] (features) and optionally qb[3..34] = J gx (directional derivative of every feature along gx); with MASK the
+// columns of levels >= n_active are written as 0 (the tensor-core forward aliases q onto the encoding rows: no stale values)
+template <bool WITH_QB, bool MASK = false>
 __device__ __forceinline__ void gather_enc(const nsr_grid_t& g, const __half2* __restrict__ table, float x, float y, float z, float gx0,
-                                           float gx1, float gx2, float (&e)[NINP], float (&qb)[NINP]) {
+                                           float gx1, float gx2, float (&e)[NINP], float (&qb)[NINP], int n_active = 16) {
 #pragma unroll
   for (int l = 0; l < 16; ++l) {
+    if (MASK && l >= n_active) {
+      e[3 + 2 * l] = e[4 + 2 * l] = 0.f;
+      if (WITH_QB) qb[3 + 2 * l] = qb[4 + 2 * l] = 0.f;
+      continue;
+    }
     const LevelInfo li = nsr_level(g, l);
     uint32_t cx, cy, cz, idx[8];
     float fx, fy, fz;
@@ -84,14 +97,16 @@ __device__ __forceinline__ void gather_enc(const nsr_grid_t& g, const __half2* _
   }
 }
 
+template <bool MASK>
 __global__ void __launch_bounds__(kThreads, 3) neus_field_fwd_kernel(const __grid_constant__ nsr_grid_t g, const float* __restrict__ points,
                                                                   const __half2* __restrict__ table, const float* __restrict__ W1,
                                                                   const float* __restrict__ b1, const float* __restrict__ W2,
                                                                   const float* __restrict__ b2, float radius, int n_out,
                                                                   float* __restrict__ sdf, float* __restrict__ grad,
                                                                   float* __restrict__ feat, int64_t n_cap,
-                                                                  const int64_t* __restrict__ n_dev) {
+                                                                  const int64_t* __restrict__ n_dev, const float* __restrict__ n_active_p) {
   const int64_t n = n_dev ? min(*n_dev, n_cap) : n_cap;
+  const int n_active = MASK ? load_n_active(n_active_p) : 16;
   __shared__ NeusW w;
   stage_neus_weights(w, W1, b1, W2, b2, n_out);
   __syncthreads();
@@ -103,7 +118,7 @@ __global__ void __launch_bounds__(kThreads, 3) neus_field_fwd_kernel(const __gri
     e[1] = 2.f * y - 1.f;
     e[2] = 2.f * z - 1.f;
     e[NIN] = 0.f;
-    gather_enc<false>(g, table, x, y, z, 0.f, 0.f, 0.f, e, dummy);
+    gather_enc<false, MASK>(g, table, x, y, z, 0.f, 0.f, 0.f, e, dummy, n_active);
     float out[NOUTP];
 #pragma unroll
     for (int o = 0; o < NOUTP; ++o) out[o] = w.b2[o];
@@ -128,10 +143,11 @@ __global__ void __launch_bounds__(kThreads, 3) neus_field_fwd_kernel(const __gri
 #pragma unroll
       for (int j = 0; j < NINP; ++j) q[j] = fmaf(row[j], u, q[j]);
     }
-    // analytic normal: second gather, features weighted by q
+    // analytic normal: second gather, features weighted by q (q of a masked level is not 0: skipped by index)
     float gx = 2.f * q[0], gy = 2.f * q[1], gz = 2.f * q[2];
 #pragma unroll
     for (int l = 0; l < 16; ++l) {
+      if (MASK && l >= n_active) break;
       const LevelInfo li = nsr_level(g, l);
       uint32_t cx, cy, cz, idx[8];
       float fx, fy, fz;
@@ -206,14 +222,16 @@ __device__ __forceinline__ void acc_to_split_afrag(const float (&acc)[1][8][4], 
     }
 }
 
+template <bool MASK>
 __global__ void __launch_bounds__(kThreads, 4) neus_field_fwd_tc_kernel(const __grid_constant__ nsr_grid_t g, const float* __restrict__ points,
                                                                         const __half2* __restrict__ table, const float* __restrict__ W1,
                                                                         const float* __restrict__ b1, const float* __restrict__ W2,
                                                                         const float* __restrict__ b2, float radius, int n_out,
                                                                         float* __restrict__ sdf, float* __restrict__ grad,
                                                                         float* __restrict__ feat, int64_t n_cap,
-                                                                        const int64_t* __restrict__ n_dev) {
+                                                                        const int64_t* __restrict__ n_dev, const float* __restrict__ n_active_p) {
   const int64_t n = n_dev ? min(*n_dev, n_cap) : n_cap;
+  const int n_active = MASK ? load_n_active(n_active_p) : 16;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   NeusTcSmem& S = *reinterpret_cast<NeusTcSmem*>(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, gq = lane >> 2, cq = lane & 3;
@@ -248,7 +266,7 @@ __global__ void __launch_bounds__(kThreads, 4) neus_field_fwd_tc_kernel(const __
       e[1] = 2.f * y - 1.f;
       e[2] = 2.f * z - 1.f;
       e[NIN] = 0.f;
-      gather_enc<false>(g, table, x, y, z, 0.f, 0.f, 0.f, e, dummy);
+      gather_enc<false, MASK>(g, table, x, y, z, 0.f, 0.f, 0.f, e, dummy, n_active);   // masked columns written as 0
       __half* rh = S.Ehi[warp][lane];
       __half* rl = S.Elo[warp][lane];
 #pragma unroll
@@ -339,6 +357,7 @@ __global__ void __launch_bounds__(kThreads, 4) neus_field_fwd_tc_kernel(const __
       float gx = 2.f * qr[0], gy = 2.f * qr[1], gz = 2.f * qr[2];
 #pragma unroll
       for (int l = 0; l < 16; ++l) {
+        if (MASK && l >= n_active) break;   // q of a masked level is a column of W1^T u, not 0
         const LevelInfo li = nsr_level(g, l);
         uint32_t cx, cy, cz, idx[8];
         float fx, fy, fz;
@@ -388,6 +407,7 @@ __device__ __forceinline__ void wgrad_block(float (&acc)[1][2][4], const __half*
   nsr_gemm_w<1, 8, 2>(acc, a, Bt + (size_t)n0 * LDT, LDT);
 }
 
+template <bool MASK>
 __global__ void __launch_bounds__(kThreads, 2) neus_field_bwd_kernel(const __grid_constant__ nsr_grid_t g, const float* __restrict__ points,
                                                                      const __half2* __restrict__ table, const float* __restrict__ W1,
                                                                      const float* __restrict__ b1, const float* __restrict__ W2,
@@ -397,8 +417,9 @@ __global__ void __launch_bounds__(kThreads, 2) neus_field_bwd_kernel(const __gri
                                                                      const float* __restrict__ amax_ptr, float* __restrict__ grad_table,
                                                                      float* __restrict__ dW1, float* __restrict__ db1, float* __restrict__ dW2,
                                                                      float* __restrict__ db2, int64_t n_cap,
-                                                                     const int64_t* __restrict__ n_dev) {
+                                                                     const int64_t* __restrict__ n_dev, const float* __restrict__ n_active_p) {
   const int64_t n = n_dev ? min(*n_dev, n_cap) : n_cap;
+  const int n_active = MASK ? load_n_active(n_active_p) : 16;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   NeusW& w = *reinterpret_cast<NeusW*>(smem_raw);
   __half* T = reinterpret_cast<__half*>(smem_raw + sizeof(NeusW));
@@ -452,7 +473,7 @@ __global__ void __launch_bounds__(kThreads, 2) neus_field_bwd_kernel(const __gri
       qb[0] = 2.f * gx0;
       qb[1] = 2.f * gx1;
       qb[2] = 2.f * gx2;
-      gather_enc<true>(g, table, x, y, z, gx0, gx1, gx2, e, qb);
+      gather_enc<true, MASK>(g, table, x, y, z, gx0, gx1, gx2, e, qb, n_active);   // e = qb = 0 on masked levels: their dW1 columns get 0
     }
 #pragma unroll 2
     for (int k = 0; k < NH; ++k) {
@@ -500,6 +521,7 @@ __global__ void __launch_bounds__(kThreads, 2) neus_field_bwd_kernel(const __gri
     constexpr int kMergeLevels = 0;
 #pragma unroll
     for (int l = 0; l < 16; ++l) {
+      if (MASK && l >= n_active) break;   // eb and q of a masked level are not 0: its table slice is left untouched
       const float eb0 = eb[3 + 2 * l], eb1 = eb[4 + 2 * l], q0 = q[3 + 2 * l], q1 = q[4 + 2 * l];
       const LevelInfo li = nsr_level(g, l);
       uint32_t cx, cy, cz, idx[8];
@@ -633,15 +655,16 @@ int check(const nsr_grid_t* g, int n_out, const char* name) {
   return 0;
 }
 
-}  // namespace
-
-extern "C" int nsr_neus_field_fwd(const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1,
-                                  const float* W2, const float* b2, float radius, int32_t n_out, float* sdf, float* grad, float* feature,
-                                  int64_t n, const int64_t* n_dev, void* stream) {
-  if (int e = check(g, n_out, "nsr_neus_field_fwd")) return e;
+// MASK selects the level-masked instantiations (n_active: device float); the unmasked ones never read it
+template <bool MASK>
+int field_fwd(const char* name, const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1, const float* W2,
+              const float* b2, float radius, int32_t n_out, const float* n_active, float* sdf, float* grad, float* feature, int64_t n,
+              const int64_t* n_dev, void* stream) {
+  if (int e = check(g, n_out, name)) return e;
+  NSR_REQUIRE(!MASK || n_active != nullptr, "%s: n_active (device float) is NULL", name);
   if (n == 0) return 0;
   // Default: neus_field_fwd_tc_kernel (SDF network on tensor cores, hi / lo split operands; same results to ~1e-6, every NeuS parity test
-  // runs on it); NSR_NEUS_FWD=scalar selects the thread-per-sample kernel.
+  // runs on it); NSR_NEUS_FWD=scalar selects the thread-per-sample kernel (masked or not, as the entry point asks).
   // The kernel is bound by the latency of its two gathers: fewer instructions only pay once the freed registers / shared memory buy a
   // fourth CTA per SM (q aliased onto the encoding rows).  Issuing the corner loads of four levels together, as the NeRF forward does,
   // was not faster and is not kept.
@@ -651,46 +674,80 @@ extern "C" int nsr_neus_field_fwd(const nsr_grid_t* g, const float* points, cons
   }();
   if (scalar) {
     const int grid = (int)min((int64_t)nsr_sm_count() * 8, (n + kThreads - 1) / kThreads);
-    neus_field_fwd_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(*g, points, (const __half2*)table_h, W1, b1, W2, b2, radius, n_out, sdf,
-                                                                       grad, feature, n, n_dev);
+    neus_field_fwd_kernel<MASK><<<grid, kThreads, 0, (cudaStream_t)stream>>>(*g, points, (const __half2*)table_h, W1, b1, W2, b2, radius, n_out,
+                                                                             sdf, grad, feature, n, n_dev, n_active);
   } else {
     static thread_local bool attr_set = false;
     if (!attr_set) {
-      cudaError_t e = cudaFuncSetAttribute(neus_field_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(NeusTcSmem));
+      cudaError_t e = cudaFuncSetAttribute(neus_field_fwd_tc_kernel<MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(NeusTcSmem));
       if (e != cudaSuccess) {
-        nsr_set_error("nsr_neus_field_fwd: cannot reserve %zu B shared memory: %s", sizeof(NeusTcSmem), cudaGetErrorString(e));
+        nsr_set_error("%s: cannot reserve %zu B shared memory: %s", name, sizeof(NeusTcSmem), cudaGetErrorString(e));
         return 2;
       }
       attr_set = true;
     }
     const int grid = (int)min((int64_t)nsr_sm_count() * 4, (n + kThreads - 1) / kThreads);
-    neus_field_fwd_tc_kernel<<<grid, kThreads, sizeof(NeusTcSmem), (cudaStream_t)stream>>>(*g, points, (const __half2*)table_h, W1, b1, W2, b2, radius,
-                                                                                            n_out, sdf, grad, feature, n, n_dev);
+    neus_field_fwd_tc_kernel<MASK><<<grid, kThreads, sizeof(NeusTcSmem), (cudaStream_t)stream>>>(*g, points, (const __half2*)table_h, W1, b1, W2,
+                                                                                                  b2, radius, n_out, sdf, grad, feature, n, n_dev,
+                                                                                                  n_active);
   }
-  NSR_CHECK_LAUNCH("nsr_neus_field_fwd");
+  NSR_CHECK_LAUNCH(name);
   return 0;
+}
+
+template <bool MASK>
+int field_bwd(const char* name, const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1, const float* W2,
+              const float* b2, float radius, int32_t n_out, const float* n_active, const float* g_out, const float* g_sdf, const float* g_grad,
+              const float* amax, float* grad_table, float* dW1, float* db1, float* dW2, float* db2, int64_t n, const int64_t* n_dev, void* stream) {
+  if (int e = check(g, n_out, name)) return e;
+  NSR_REQUIRE(!MASK || n_active != nullptr, "%s: n_active (device float) is NULL", name);
+  if (n == 0) return 0;
+  static thread_local bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(neus_field_bwd_kernel<MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmem);
+    if (e != cudaSuccess) {
+      nsr_set_error("%s: cannot reserve %zu B shared memory: %s", name, kBwdSmem, cudaGetErrorString(e));
+      return 2;
+    }
+    attr_set = true;
+  }
+  const int grid = (int)min((int64_t)nsr_sm_count() * 2, (n + kThreads - 1) / kThreads);  // two CTAs per SM: their gather / MLP / scatter phases overlap
+  neus_field_bwd_kernel<MASK><<<grid, kThreads, kBwdSmem, (cudaStream_t)stream>>>(*g, points, (const __half2*)table_h, W1, b1, W2, b2, radius, n_out,
+                                                                                  g_out, g_sdf, g_grad, amax, grad_table, dW1, db1, dW2, db2, n, n_dev,
+                                                                                  n_active);
+  NSR_CHECK_LAUNCH(name);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int nsr_neus_field_fwd(const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1,
+                                  const float* W2, const float* b2, float radius, int32_t n_out, float* sdf, float* grad, float* feature,
+                                  int64_t n, const int64_t* n_dev, void* stream) {
+  return field_fwd<false>("nsr_neus_field_fwd", g, points, table_h, W1, b1, W2, b2, radius, n_out, nullptr, sdf, grad, feature, n, n_dev, stream);
 }
 
 extern "C" int nsr_neus_field_bwd(const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1,
                                   const float* W2, const float* b2, float radius, int32_t n_out, const float* g_out, const float* g_sdf,
                                   const float* g_grad, const float* amax, float* grad_table, float* dW1, float* db1, float* dW2, float* db2, int64_t n,
                                   const int64_t* n_dev, void* stream) {
-  if (int e = check(g, n_out, "nsr_neus_field_bwd")) return e;
-  if (n == 0) return 0;
-  static thread_local bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(neus_field_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmem);
-    if (e != cudaSuccess) {
-      nsr_set_error("nsr_neus_field_bwd: cannot reserve %zu B shared memory: %s", kBwdSmem, cudaGetErrorString(e));
-      return 2;
-    }
-    attr_set = true;
-  }
-  const int grid = (int)min((int64_t)nsr_sm_count() * 2, (n + kThreads - 1) / kThreads);  // two CTAs per SM: their gather / MLP / scatter phases overlap
-  neus_field_bwd_kernel<<<grid, kThreads, kBwdSmem, (cudaStream_t)stream>>>(*g, points, (const __half2*)table_h, W1, b1, W2, b2, radius, n_out,
-                                                                            g_out, g_sdf, g_grad, amax, grad_table, dW1, db1, dW2, db2, n, n_dev);
-  NSR_CHECK_LAUNCH("nsr_neus_field_bwd");
-  return 0;
+  return field_bwd<false>("nsr_neus_field_bwd", g, points, table_h, W1, b1, W2, b2, radius, n_out, nullptr, g_out, g_sdf, g_grad, amax, grad_table,
+                          dW1, db1, dW2, db2, n, n_dev, stream);
+}
+
+extern "C" int nsr_neus_field_fwd_levels(const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1,
+                                         const float* W2, const float* b2, float radius, int32_t n_out, const float* n_active, float* sdf,
+                                         float* grad, float* feature, int64_t n, const int64_t* n_dev, void* stream) {
+  return field_fwd<true>("nsr_neus_field_fwd_levels", g, points, table_h, W1, b1, W2, b2, radius, n_out, n_active, sdf, grad, feature, n, n_dev,
+                         stream);
+}
+
+extern "C" int nsr_neus_field_bwd_levels(const nsr_grid_t* g, const float* points, const void* table_h, const float* W1, const float* b1,
+                                         const float* W2, const float* b2, float radius, int32_t n_out, const float* n_active, const float* g_out,
+                                         const float* g_sdf, const float* g_grad, const float* amax, float* grad_table, float* dW1, float* db1,
+                                         float* dW2, float* db2, int64_t n, const int64_t* n_dev, void* stream) {
+  return field_bwd<true>("nsr_neus_field_bwd_levels", g, points, table_h, W1, b1, W2, b2, radius, n_out, n_active, g_out, g_sdf, g_grad, amax,
+                         grad_table, dW1, db1, dW2, db2, n, n_dev, stream);
 }
 
 namespace {

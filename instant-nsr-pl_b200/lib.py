@@ -98,6 +98,8 @@ _SIGNATURES = {
     'nsr_nerf_rays_bwd': [P, P, P, P, P, F32, P, P, P, P, P, P, P, P, P, P, P, P, P, P, F32, P, F32, P, I64, P],
     'nsr_neus_field_fwd': [P, P, P, P, P, P, P, F32, I32, P, P, P, I64, P, P],
     'nsr_neus_field_bwd': [P, P, P, P, P, P, P, F32, I32, P, P, P, P, P, P, P, P, P, I64, P, P],
+    'nsr_neus_field_fwd_levels': [P, P, P, P, P, P, P, F32, I32, P, P, P, P, I64, P, P],
+    'nsr_neus_field_bwd_levels': [P, P, P, P, P, P, P, F32, I32, P, P, P, P, P, P, P, P, P, P, I64, P, P],
     'nsr_neus_field_fd_fwd': [P, P, P, P, P, P, P, F32, I32, P, P, P, P, P, I64, P, P],
     'nsr_neus_field_fd_bwd': [P, P, P, P, P, P, P, F32, I32, P, P, P, P, P, P, P, P, P, P, I64, P, P],
     'nsr_absmax3': [P, I64, P, I64, P, I64, P, I64, P, P],

@@ -90,27 +90,33 @@ class VolumeSDF(BaseImplicitGeometry):
         self.n_output_dims = self.config.feature_dim
         self.encoding = get_encoding(3, self.config.xyz_encoding_config)
         self.network = get_mlp(self.encoding.n_output_dims, self.n_output_dims, self.config.mlp_network_config)
+        from .networks import ProgressiveBandHashGrid
+        self._progressive = isinstance(self.encoding.encoding, ProgressiveBandHashGrid)
         self.grad_type = self.config.grad_type
         self.finite_difference_eps = self.config.get('finite_difference_eps', 1e-3)
         self._finite_difference_eps = None  # value in use; updated per step when "progressive"
         self._fused = self.config.get('fused', True) and self._fusable()
         self._fused_fd = self.config.get('fused', True) and self._fusable_fd()
-        # {eps, eps^2, n_active} on the device for the finite-difference kernels; update_step refreshes it in place, so a captured
-        # CUDA graph follows the schedule
+        # {eps, eps^2, n_active} on the device for the finite-difference kernels (n_active alone for the analytic kernels under a
+        # ProgressiveBandHashGrid); update_step refreshes it in place, so a captured CUDA graph follows the schedule
         # (a ProgressiveBandHashGrid masks every level until its first update_step)
-        from .networks import ProgressiveBandHashGrid
-        n_active = 0.0 if isinstance(self.encoding.encoding, ProgressiveBandHashGrid) else 16.0
+        n_active = 0.0 if self._progressive else 16.0
         self.register_buffer('_fd_state', torch.tensor([float('nan'), float('nan'), n_active]), persistent=False)
 
     def _fusable(self):
         """the neus-blender / neus-dtu geometry shape (configs/neus-blender.yaml:36-63): include_xyz HashGrid(L=16, F=2) + VanillaMLP
-        35 -> 64 (Softplus 100) -> n_out <= 16 with analytic normals => one fused forward and one fused backward kernel"""
+        35 -> 64 (Softplus 100) -> n_out <= 16 with analytic normals => one fused forward and one fused backward kernel.  With the
+        opt-in key ``fused_progressive: true`` the same grid inside a ProgressiveBandHashGrid (neus-colmap) is fusable too: the kernels
+        then mask the hash levels >= current_level (nsr_neus_field_*_levels)."""
         from .. import tcnn
         from .networks import VanillaMLP
-        enc, net = self.encoding, self.network
+        net = self.network
+        if self._progressive and not self.config.get('fused_progressive', False):
+            return False
         try:
-            return (self.grad_type == 'analytic' and enc.include_xyz and isinstance(enc.encoding, tcnn.Encoding)
-                    and enc.encoding.grid is not None and enc.encoding.grid.n_levels == 16 and enc.encoding.grid.n_features == 2
+            enc = self._fd_grid()
+            return (self.grad_type == 'analytic' and self.encoding.include_xyz and isinstance(enc, tcnn.Encoding)
+                    and enc.grid is not None and enc.grid.n_levels == 16 and enc.grid.n_features == 2
                     and isinstance(net, VanillaMLP) and net.n_hidden_layers == 1 and net.n_neurons == 64 and net.sphere_init
                     and self.config.mlp_network_config.get('output_activation', 'none') in (None, 'none') and self.n_output_dims <= 16
                     and 'sdf_activation' not in self.config and 'feature_activation' not in self.config)
@@ -118,10 +124,9 @@ class VolumeSDF(BaseImplicitGeometry):
             return False
 
     def _fd_grid(self):
-        """the tcnn.Encoding under the include_xyz wrapper (inside a ProgressiveBandHashGrid for the Neuralangelo config)"""
-        from .networks import ProgressiveBandHashGrid
+        """the tcnn.Encoding under the include_xyz wrapper (inside a ProgressiveBandHashGrid for the Neuralangelo and neus-colmap configs)"""
         inner = self.encoding.encoding
-        return inner.encoding if isinstance(inner, ProgressiveBandHashGrid) else inner
+        return inner.encoding if self._progressive else inner
 
     def _fusable_fd(self):
         """the Neuralangelo geometry shape (configs/neuralangelo-dtu-wmask.yaml:18-75): include_xyz HashGrid or ProgressiveBandHashGrid
@@ -141,9 +146,7 @@ class VolumeSDF(BaseImplicitGeometry):
             return False
 
     def _n_active_levels(self):
-        from .networks import ProgressiveBandHashGrid
-        inner = self.encoding.encoding
-        return int(inner.current_level) if isinstance(inner, ProgressiveBandHashGrid) else 16
+        return int(self.encoding.encoding.current_level) if self._progressive else 16
 
     def _effective_weights(self):
         ws = []
@@ -158,11 +161,13 @@ class VolumeSDF(BaseImplicitGeometry):
     def _forward_fused(self, points, with_grad, with_feature):
         from .. import ops
         from ..nerfacc import ContractionType
-        enc = self.encoding.encoding
+        enc = self._fd_grid()
         shape = points.shape[:-1]
         W1, b1, W2, b2 = self._effective_weights()
+        n_active = self._fd_state[2:] if self._progressive else None   # device word: a captured graph follows the level schedule
         with torch.set_grad_enabled(self.training and torch.is_grad_enabled()):
-            sdf, grad, feat = ops.neus_sdf(enc.grid, self.radius, points.reshape(-1, 3), enc.params, enc._params_half(), W1, b1, W2, b2)
+            sdf, grad, feat = ops.neus_sdf(enc.grid, self.radius, points.reshape(-1, 3), enc.params, enc._params_half(), W1, b1, W2, b2,
+                                           n_active=n_active)
         rv = [sdf.reshape(shape)]
         if with_grad:
             rv.append(grad.reshape(*shape, 3))
@@ -254,6 +259,8 @@ class VolumeSDF(BaseImplicitGeometry):
         update_module_step(self.encoding, epoch, global_step)
         update_module_step(self.network, epoch, global_step)
         if self.grad_type != 'finite_difference':
+            if self._progressive:   # the analytic kernels' level mask, in place like the finite-difference state below
+                self._fd_state[2:3].fill_(float(self._n_active_levels()))
             return
         if isinstance(self.finite_difference_eps, float):
             self._finite_difference_eps = self.finite_difference_eps

@@ -189,7 +189,8 @@ class NeuSModel(BaseModel):
             if not (getattr(self.geometry, '_fused', False) or getattr(self.geometry, '_fused_fd', False)):
                 raise NotImplementedError('static NeuS forward with a learned background: needs the fused foreground SDF field (include_xyz '
                                           'HashGrid + sphere-init VanillaMLP, analytic or finite-difference normals); a ProgressiveBandHashGrid '
-                                          'with analytic normals (neus-colmap) runs the per-op field')
+                                          'with analytic normals (neus-colmap) runs the per-op field unless the geometry sets '
+                                          'fused_progressive: true')
             missing = NerfBackgroundFused.unsupported(self)
             if missing is not None:
                 raise NotImplementedError(f'static NeuS forward with a learned background: needs {missing}')

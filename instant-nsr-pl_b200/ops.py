@@ -532,15 +532,20 @@ class _NeusSDF(torch.autograd.Function):
     the second-order terms the eikonal / normal-dependent losses need are inside nsr_neus_field_bwd."""
 
     @staticmethod
-    def forward(ctx, spec, radius, n_out, points, table_f32, table_h, W1, b1, W2, b2):
+    def forward(ctx, spec, radius, n_out, points, table_f32, table_h, W1, b1, W2, b2, n_active):
         n = points.shape[0]
         dev = points.device
         sdf = torch.empty(n, device=dev)
         grad = torch.empty(n, 3, device=dev)
         feat = torch.empty(n, n_out, device=dev)
-        lib.call('nsr_neus_field_fwd', spec.ref(), ptr(points), ptr(table_h), ptr(W1), ptr(b1), ptr(W2), ptr(b2), float(radius), int(n_out),
-                 ptr(sdf), ptr(grad), ptr(feat), n, ptr(_LIVE_ROWS), stream())
+        if n_active is None:
+            lib.call('nsr_neus_field_fwd', spec.ref(), ptr(points), ptr(table_h), ptr(W1), ptr(b1), ptr(W2), ptr(b2), float(radius), int(n_out),
+                     ptr(sdf), ptr(grad), ptr(feat), n, ptr(_LIVE_ROWS), stream())
+        else:
+            lib.call('nsr_neus_field_fwd_levels', spec.ref(), ptr(points), ptr(table_h), ptr(W1), ptr(b1), ptr(W2), ptr(b2), float(radius),
+                     int(n_out), ptr(n_active), ptr(sdf), ptr(grad), ptr(feat), n, ptr(_LIVE_ROWS), stream())
         ctx.spec, ctx.radius, ctx.n_out, ctx.k_dev = spec, radius, n_out, _LIVE_ROWS
+        ctx.n_active = n_active
         ctx.save_for_backward(points, table_h, W1, b1, W2, b2)
         return sdf, grad, feat
 
@@ -556,18 +561,27 @@ class _NeusSDF(torch.autograd.Function):
         sizes = [W1.numel(), b1.numel(), W2.numel(), b2.numel()]
         flat = torch.zeros(sum(sizes), device=dev)   # one fill for the four small gradients
         dW1, db1, dW2, db2 = [t.view_as(w) for t, w in zip(flat.split(sizes), (W1, b1, W2, b2))]
-        lib.call('nsr_neus_field_bwd', ctx.spec.ref(), ptr(points), ptr(table_h), ptr(W1), ptr(b1), ptr(W2), ptr(b2), float(ctx.radius),
-                 int(n_out), ptr(g_feat), ptr(g_sdf), ptr(g_grad), ptr(amax), ptr(dtable), ptr(dW1), ptr(db1), ptr(dW2), ptr(db2), n, ptr(ctx.k_dev),
-                 stream())
-        return None, None, None, None, dtable, None, dW1, db1, dW2, db2
+        if ctx.n_active is None:
+            lib.call('nsr_neus_field_bwd', ctx.spec.ref(), ptr(points), ptr(table_h), ptr(W1), ptr(b1), ptr(W2), ptr(b2), float(ctx.radius),
+                     int(n_out), ptr(g_feat), ptr(g_sdf), ptr(g_grad), ptr(amax), ptr(dtable), ptr(dW1), ptr(db1), ptr(dW2), ptr(db2), n,
+                     ptr(ctx.k_dev), stream())
+        else:
+            lib.call('nsr_neus_field_bwd_levels', ctx.spec.ref(), ptr(points), ptr(table_h), ptr(W1), ptr(b1), ptr(W2), ptr(b2), float(ctx.radius),
+                     int(n_out), ptr(ctx.n_active), ptr(g_feat), ptr(g_sdf), ptr(g_grad), ptr(amax), ptr(dtable), ptr(dW1), ptr(db1), ptr(dW2),
+                     ptr(db2), n, ptr(ctx.k_dev), stream())
+        return None, None, None, None, dtable, None, dW1, db1, dW2, db2, None
 
 
-def neus_sdf(spec, radius, points, table_f32, table_h, W1, b1, W2, b2):
-    """points [N,3] world (AABB scene of half-extent `radius`); W1 [64,35], b1 [64], W2 [n_out,64], b2 [n_out] fp32 (effective weights)."""
-    check_cuda(points, table_h, W1, W2, what='VolumeSDF (fused)')
+def neus_sdf(spec, radius, points, table_f32, table_h, W1, b1, W2, b2, n_active=None):
+    """points [N,3] world (AABB scene of half-extent `radius`); W1 [64,35], b1 [64], W2 [n_out,64], b2 [n_out] fp32 (effective weights).
+    n_active: None (all 16 hash levels), or a float32 CUDA tensor of one entry -- the ProgressiveBandHashGrid level count, read on the
+    device by the kernels (levels >= n_active contribute 0), so an in-place update reaches a captured CUDA graph."""
+    check_cuda(points, table_h, W1, W2, n_active, what='VolumeSDF (fused)')
+    if n_active is not None and (n_active.dtype != torch.float32 or n_active.numel() != 1):
+        raise ValueError('n_active must be a float32 tensor of one entry (the number of active hash levels)')
     n_out = W2.shape[0]
     return _NeusSDF.apply(spec, float(radius), int(n_out), contig(points.detach(), torch.float32), table_f32, table_h,
-                          contig(W1, torch.float32), contig(b1, torch.float32), contig(W2, torch.float32), contig(b2, torch.float32))
+                          contig(W1, torch.float32), contig(b1, torch.float32), contig(W2, torch.float32), contig(b2, torch.float32), n_active)
 
 
 class _NeusSDFFd(torch.autograd.Function):
