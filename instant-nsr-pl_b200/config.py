@@ -43,22 +43,3 @@ def to_primitive(c):
     if isinstance(c, (list, tuple)):
         return [to_primitive(v) for v in c]
     return c
-
-
-# kernel paths seen green in the GPU suite: on by default, NSR_DISABLE=name[,name] switches one off again
-VALIDATED = {'mlp_vanilla', 'radiance_vanilla', 'pack_scan'}
-
-
-def experimental(name):
-    """True when the kernel path ``name`` is switched on.  Paths in VALIDATED are on unless NSR_DISABLE lists them; any other name is a
-    path that has not passed the GPU suite yet and stays off unless the environment asks for it: NSR_EXPERIMENTAL=1 (all) or a comma-separated
-    list of names."""
-    import os
-    if name in [x.strip() for x in os.environ.get('NSR_DISABLE', '').split(',') if x.strip()]:
-        return False
-    if name in VALIDATED:
-        return True
-    v = os.environ.get('NSR_EXPERIMENTAL', '').strip()
-    if v in ('', '0'):
-        return False
-    return v == '1' or name in [x.strip() for x in v.split(',')]

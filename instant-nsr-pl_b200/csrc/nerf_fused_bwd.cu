@@ -9,7 +9,6 @@
 // kernel; one atomicAdd per weight per CTA at the end (tcnn: split-K CUTLASS GEMMs over K = batch + reduction).
 // The split backward's network half (nerf_bwd_net_kernel, below) runs the same chain but hands the weight-gradient GEMMs to a wgmma
 // warpgroup.
-#include <stdlib.h>
 #include "nerf_fused.cuh"
 #include "wgmma.cuh"
 
@@ -713,8 +712,8 @@ namespace {
 // this form against the plain 8-byte REDs).
 constexpr int kMergeLevels = 8;
 
-template <int MINB>   // resident CTAs per SM the register allocation is sized for: 5 (48 registers), 6 (40), 8 (32, 64 B of spills)
-__global__ void __launch_bounds__(256, MINB) nerf_table_scatter_kernel(const __grid_constant__ nsr_grid_t g, const float* __restrict__ xyz, int stride,
+// The register allocation is sized for 5 resident CTAs per SM (48 registers); budgets for 6 and 8 CTAs spill and measured slower.
+__global__ void __launch_bounds__(256, 5) nerf_table_scatter_kernel(const __grid_constant__ nsr_grid_t g, const float* __restrict__ xyz, int stride,
                                                                  const __half2* __restrict__ denc, float loss_scale,
                                                                  const float* __restrict__ amax_ptr, float* __restrict__ grad_table,
                                                                  int64_t n_cap, const int64_t* __restrict__ n_dev, int l_begin, int l_end) {
@@ -942,20 +941,8 @@ extern "C" int nsr_nerf_table_scatter(const nsr_grid_t* g, const float* xyz, int
   if (k == 0 || level_begin == level_end) return 0;
   const int per_sm = ctas_per_sm >= 1 && ctas_per_sm <= 8 ? ctas_per_sm : 8;   // < 8 leaves room for a kernel running beside it (the exchange)
   const int grid = (int)min((int64_t)nsr_sm_count() * per_sm, (k + 255) / 256);
-  static const int occ = [] {   // NSR_SCATTER_CTAS = 5 (default) | 6 | 8: register budget of the instantiation
-    const char* v = getenv("NSR_SCATTER_CTAS");
-    const int n = v ? atoi(v) : 5;
-    return n == 6 || n == 8 ? n : 5;
-  }();
-  const int g_ = k_dev ? nsr_sm_count() * per_sm : grid;
-  cudaStream_t st_ = (cudaStream_t)stream;
-  const __half2* de_ = (const __half2*)denc_h;
-  if (occ == 6)
-    nerf_table_scatter_kernel<6><<<g_, 256, 0, st_>>>(*g, xyz, stride, de_, loss_scale, amax, grad_table, k, k_dev, level_begin, level_end);
-  else if (occ == 8)
-    nerf_table_scatter_kernel<8><<<g_, 256, 0, st_>>>(*g, xyz, stride, de_, loss_scale, amax, grad_table, k, k_dev, level_begin, level_end);
-  else
-    nerf_table_scatter_kernel<5><<<g_, 256, 0, st_>>>(*g, xyz, stride, de_, loss_scale, amax, grad_table, k, k_dev, level_begin, level_end);
+  nerf_table_scatter_kernel<<<k_dev ? nsr_sm_count() * per_sm : grid, 256, 0, (cudaStream_t)stream>>>(*g, xyz, stride, (const __half2*)denc_h, loss_scale,
+                                                                                                  amax, grad_table, k, k_dev, level_begin, level_end);
   NSR_CHECK_LAUNCH("nsr_nerf_table_scatter");
   return 0;
 }
@@ -970,7 +957,7 @@ extern "C" int nsr_nerf_field_bwd_split(const nsr_nerf_t* f, const void* enc_k_h
                                       denc_h, stream, "nsr_nerf_field_bwd_split");
   if (rc != 0 || k == 0) return rc;
   const int grid = (int)min((int64_t)nsr_sm_count() * 8, (k + 255) / 256);
-  nerf_table_scatter_kernel<5><<<k_dev ? nsr_sm_count() * 8 : grid, 256, 0, (cudaStream_t)stream>>>(f->grid, xyzdir, 6, (const __half2*)denc_h, loss_scale, amax,
+  nerf_table_scatter_kernel<<<k_dev ? nsr_sm_count() * 8 : grid, 256, 0, (cudaStream_t)stream>>>(f->grid, xyzdir, 6, (const __half2*)denc_h, loss_scale, amax,
                                                                                                  grad_dparams + NF_DENSITY_PARAMS, k, k_dev, 0, 16);
   NSR_CHECK_LAUNCH("nsr_nerf_field_bwd_split (scatter)");
   return 0;

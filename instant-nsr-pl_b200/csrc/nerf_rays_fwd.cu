@@ -11,7 +11,6 @@
 // expand kernels.  Per-ray outputs are plain stores (no atomics: bit-reproducible); kept samples of ray r land at
 // offsets_m[r] + j (j < kept[r]) in the per-sample buffers ("loose" layout: a kept prefix per ray).
 // The kept set is identical to the two-pass path: same density code, same 32-sample chunking of the scan.
-#include <stdlib.h>
 #include "nerf_fused.cuh"
 
 namespace {
@@ -64,10 +63,12 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
-// MINB = resident CTAs per SM the register allocation is sized for: 2 (128 registers).  (A 3-CTA instantiation -- 80 registers, 0.5 KB of
-// spills per thread, 24 warps per SM -- was markedly slower and is not built.)
-template <int MINB, int NB>
-__global__ void __launch_bounds__(kThreads, MINB) nerf_rays_fwd_kernel(const __grid_constant__ nsr_nerf_t P, const RaysFwdArgs a) {
+// The register allocation is sized for kMinBlocks resident CTAs per SM: 2 (128 registers).  (3 CTAs -- 80 registers, 0.5 KB of spills per
+// thread, 24 warps per SM -- was markedly slower.)
+constexpr int kMinBlocks = 2;
+// levels whose 8 corner loads are issued together (8 levels measured no faster and spilled 120 B)
+constexpr int kGatherBatch = 4;
+__global__ void __launch_bounds__(kThreads, kMinBlocks) nerf_rays_fwd_kernel(const __grid_constant__ nsr_nerf_t P, const RaysFwdArgs a) {
   extern __shared__ __align__(16) __half smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
   __half* At = smem + NF_W_TOTAL + warp * kWarpHalves;
@@ -153,7 +154,7 @@ __global__ void __launch_bounds__(kThreads, MINB) nerf_rays_fwd_kernel(const __g
         if (valid) {
           const float x = (fmaf(dx, mid, ox) + P.radius) * inv, y = (fmaf(dy, mid, oy) + P.radius) * inv,
                       z = (fmaf(dz, mid, oz) + P.radius) * inv;
-          nf_gather_batched<16, NB>(P.grid, table, x, y, z, f);   // NB levels = 8 NB loads per lane in flight
+          nf_gather_batched<16, kGatherBatch>(P.grid, table, x, y, z, f);   // 8 kGatherBatch loads per lane in flight
         } else {
 #pragma unroll
           for (int l = 0; l < 16; ++l) f[l] = 0u;
@@ -426,14 +427,9 @@ extern "C" int nsr_nerf_rays_fwd(const nsr_nerf_t* f, const float* rays, const u
   NSR_REQUIRE(words >= 1 && words <= kMaxWords, "nsr_nerf_rays_fwd: words must be in [1,%d]", kMaxWords);
   NSR_REQUIRE(ticket != nullptr && kept != nullptr, "nsr_nerf_rays_fwd: ticket / kept are required");
   if (n_rays == 0) return 0;
-  static const int gather_batch = [] {   // levels whose 8 corner loads are issued together: 4 (default) or 8 (NSR_FWD_BATCH=8; 120 B of spills)
-    const char* v = getenv("NSR_FWD_BATCH");
-    return (v != nullptr && v[0] == '8') ? 8 : 4;
-  }();
   static thread_local bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(nerf_rays_fwd_kernel<2, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(nerf_rays_fwd_kernel<2, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(nerf_rays_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     if (e != cudaSuccess) {
       nsr_set_error("nsr_nerf_rays_fwd: cannot reserve %zu B shared memory: %s", kSmemBytes, cudaGetErrorString(e));
       return 2;
@@ -448,10 +444,7 @@ extern "C" int nsr_nerf_rays_fwd(const nsr_nerf_t* f, const float* rays, const u
   a.step = step; a.early_stop_eps = early_stop_eps; a.words = words; a.n_rays = n_rays;
   const int64_t want = (n_rays + kWarps - 1) / kWarps;
   int grid = (int)min((int64_t)nsr_sm_count() * 2, want > 0 ? want : (int64_t)1);
-  if (gather_batch == 8)
-    nerf_rays_fwd_kernel<2, 8><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(*f, a);
-  else
-    nerf_rays_fwd_kernel<2, 4><<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(*f, a);
+  nerf_rays_fwd_kernel<<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(*f, a);
   NSR_CHECK_LAUNCH("nsr_nerf_rays_fwd");
   return 0;
 }

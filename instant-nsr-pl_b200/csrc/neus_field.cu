@@ -8,9 +8,9 @@
 //   backward(g_out, g_grad): gx = g_grad / (2r);  qb = [2 gx | J gx];  ub = W1 qb;  zb = (W2^T g_out) s + ub W2[0] beta s (1 - s)
 //     eb = W1^T zb;  dW1 = u qb^T + zb e^T;  db1 = zb;  dW2 = g_out h^T (+ row 0: ub s);  db2 = g_out
 //     dtable[c] += w_c eb_l + q_l scale_l (dw_c/dx . gx)        (ONE 8-byte RED per corner carries both orders)
-// The SDF branch stays fp32 on the CUDA cores (the reference runs it under autocast(False): the NeuS alpha multiplies sdf by
-// inv_s up to 1e3+), weights broadcast from shared memory; only the weight-gradient outer products go through tensor cores.
-#include <stdlib.h>
+// The SDF branch keeps fp32 accuracy (the reference runs it under autocast(False): the NeuS alpha multiplies sdf by inv_s up to 1e3+):
+// the forward's products run on tensor cores with operands split into fp16 hi + lo parts (below); the backward stays on the CUDA cores,
+// weights broadcast from shared memory, and only its weight-gradient outer products go through tensor cores.
 #include "mlp_warp.cuh"
 
 namespace {
@@ -97,93 +97,13 @@ __device__ __forceinline__ void gather_enc(const nsr_grid_t& g, const __half2* _
   }
 }
 
-template <bool MASK>
-__global__ void __launch_bounds__(kThreads, 3) neus_field_fwd_kernel(const __grid_constant__ nsr_grid_t g, const float* __restrict__ points,
-                                                                  const __half2* __restrict__ table, const float* __restrict__ W1,
-                                                                  const float* __restrict__ b1, const float* __restrict__ W2,
-                                                                  const float* __restrict__ b2, float radius, int n_out,
-                                                                  float* __restrict__ sdf, float* __restrict__ grad,
-                                                                  float* __restrict__ feat, int64_t n_cap,
-                                                                  const int64_t* __restrict__ n_dev, const float* __restrict__ n_active_p) {
-  const int64_t n = n_dev ? min(*n_dev, n_cap) : n_cap;
-  const int n_active = MASK ? load_n_active(n_active_p) : 16;
-  __shared__ NeusW w;
-  stage_neus_weights(w, W1, b1, W2, b2, n_out);
-  __syncthreads();
-  const float inv2r = 1.f / (2.f * radius);
-  for (int64_t i = blockIdx.x * (int64_t)kThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kThreads) {
-    const float x = (points[i * 3 + 0] + radius) * inv2r, y = (points[i * 3 + 1] + radius) * inv2r, z = (points[i * 3 + 2] + radius) * inv2r;
-    float e[NINP], q[NINP], dummy[NINP];
-    e[0] = 2.f * x - 1.f;
-    e[1] = 2.f * y - 1.f;
-    e[2] = 2.f * z - 1.f;
-    e[NIN] = 0.f;
-    gather_enc<false, MASK>(g, table, x, y, z, 0.f, 0.f, 0.f, e, dummy, n_active);
-    float out[NOUTP];
-#pragma unroll
-    for (int o = 0; o < NOUTP; ++o) out[o] = w.b2[o];
-#pragma unroll
-    for (int j = 0; j < NINP; ++j) q[j] = 0.f;
-#pragma unroll 1
-    for (int k = 0; k < NH; ++k) {
-      float row[NINP];
-#pragma unroll
-      for (int v = 0; v < NINP / 4; ++v) *reinterpret_cast<float4*>(&row[4 * v]) = *reinterpret_cast<const float4*>(&w.W1[k][4 * v]);
-      float zk = w.b1[k];
-#pragma unroll
-      for (int j = 0; j < NINP; ++j) zk = fmaf(row[j], e[j], zk);
-      float s;
-      const float h = softplus100(zk, s);
-      float w2[NOUTP];
-#pragma unroll
-      for (int v = 0; v < NOUTP / 4; ++v) *reinterpret_cast<float4*>(&w2[4 * v]) = *reinterpret_cast<const float4*>(&w.W2T[k][4 * v]);
-#pragma unroll
-      for (int o = 0; o < NOUTP; ++o) out[o] = fmaf(w2[o], h, out[o]);
-      const float u = s * w2[0];
-#pragma unroll
-      for (int j = 0; j < NINP; ++j) q[j] = fmaf(row[j], u, q[j]);
-    }
-    // analytic normal: second gather, features weighted by q (q of a masked level is not 0: skipped by index)
-    float gx = 2.f * q[0], gy = 2.f * q[1], gz = 2.f * q[2];
-#pragma unroll
-    for (int l = 0; l < 16; ++l) {
-      if (MASK && l >= n_active) break;
-      const LevelInfo li = nsr_level(g, l);
-      uint32_t cx, cy, cz, idx[8];
-      float fx, fy, fz;
-      nsr_pos_fract(x, li.scale, cx, fx);
-      nsr_pos_fract(y, li.scale, cy, fy);
-      nsr_pos_fract(z, li.scale, cz, fz);
-      nsr_corner_indices(li, cx, cy, cz, idx);
-      float lx = 0.f, ly = 0.f, lz = 0.f;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        const float2 v = nsr_ld_table(table, idx[c]);
-        const float sv = v.x * q[3 + 2 * l] + v.y * q[4 + 2 * l];
-        lx = fmaf(nsr_corner_dweight(c, 0, fx, fy, fz), sv, lx);
-        ly = fmaf(nsr_corner_dweight(c, 1, fx, fy, fz), sv, ly);
-        lz = fmaf(nsr_corner_dweight(c, 2, fx, fy, fz), sv, lz);
-      }
-      gx = fmaf(li.scale, lx, gx);
-      gy = fmaf(li.scale, ly, gy);
-      gz = fmaf(li.scale, lz, gz);
-    }
-    sdf[i] = out[0];
-    grad[i * 3 + 0] = gx * inv2r;
-    grad[i * 3 + 1] = gy * inv2r;
-    grad[i * 3 + 2] = gz * inv2r;
-#pragma unroll
-    for (int o = 0; o < NOUTP; ++o)
-      if (o < n_out) feat[i * n_out + o] = out[o];
-  }
-}
-
 // ---- forward with the three GEMMs of the SDF network on tensor cores ---------------------------------------------------------
-// The thread-per-sample kernel above spends more than half of its instructions on the 64 x (36 + 16 + 36) scalar FMAs of  z = W1 e,  out = W2 h,  q = W1^T u  with their weight loads from shared memory.
+// As scalar FMAs, the 64 x (36 + 16 + 36) products  z = W1 e,  out = W2 h,  q = W1^T u  and their weight loads from shared memory
+// would be more than half of the forward's instructions.
 // Here a warp owns 32 samples; the gathers stay thread-per-sample, the three products run as m16n8k16 MMAs with fp32 accumulation on
 // operands SPLIT into fp16 hi + lo parts (x = hi + lo, hi = fp16(x), lo = fp16(x - hi)):  x w ~= hi_x hi_w + lo_x hi_w + hi_x lo_w, i.e.
 // ~21 bits of every product survive (the dropped lo_x lo_w term is 2^-22 relative): fp32-level accuracy for the inv_s-amplified SDF,
-// which a single fp16 product (11 bits) would not give.  Same outputs as the scalar kernel to ~1e-6 relative.
+// which a single fp16 product (11 bits) would not give.  Same outputs as fp32 FMAs to ~1e-6 relative.
 constexpr int TC_K1 = 48;              // 35 inputs padded to three k16 steps
 constexpr int TC_LD1 = TC_K1 + 8;      // 56 halves per row of the E / W1 tiles (ldmatrix conflict-free)
 
@@ -663,34 +583,22 @@ int field_fwd(const char* name, const nsr_grid_t* g, const float* points, const 
   if (int e = check(g, n_out, name)) return e;
   NSR_REQUIRE(!MASK || n_active != nullptr, "%s: n_active (device float) is NULL", name);
   if (n == 0) return 0;
-  // Default: neus_field_fwd_tc_kernel (SDF network on tensor cores, hi / lo split operands; same results to ~1e-6, every NeuS parity test
-  // runs on it); NSR_NEUS_FWD=scalar selects the thread-per-sample kernel (masked or not, as the entry point asks).
+  // neus_field_fwd_tc_kernel: the SDF network on tensor cores, hi / lo split operands.
   // The kernel is bound by the latency of its two gathers: fewer instructions only pay once the freed registers / shared memory buy a
   // fourth CTA per SM (q aliased onto the encoding rows).  Issuing the corner loads of four levels together, as the NeRF forward does,
   // was not faster and is not kept.
-  static const bool scalar = [] {
-    const char* v = getenv("NSR_NEUS_FWD");
-    return v != nullptr && v[0] == 's';
-  }();
-  if (scalar) {
-    const int grid = (int)min((int64_t)nsr_sm_count() * 8, (n + kThreads - 1) / kThreads);
-    neus_field_fwd_kernel<MASK><<<grid, kThreads, 0, (cudaStream_t)stream>>>(*g, points, (const __half2*)table_h, W1, b1, W2, b2, radius, n_out,
-                                                                             sdf, grad, feature, n, n_dev, n_active);
-  } else {
-    static thread_local bool attr_set = false;
-    if (!attr_set) {
-      cudaError_t e = cudaFuncSetAttribute(neus_field_fwd_tc_kernel<MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(NeusTcSmem));
-      if (e != cudaSuccess) {
-        nsr_set_error("%s: cannot reserve %zu B shared memory: %s", name, sizeof(NeusTcSmem), cudaGetErrorString(e));
-        return 2;
-      }
-      attr_set = true;
+  static thread_local bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(neus_field_fwd_tc_kernel<MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(NeusTcSmem));
+    if (e != cudaSuccess) {
+      nsr_set_error("%s: cannot reserve %zu B shared memory: %s", name, sizeof(NeusTcSmem), cudaGetErrorString(e));
+      return 2;
     }
-    const int grid = (int)min((int64_t)nsr_sm_count() * 4, (n + kThreads - 1) / kThreads);
-    neus_field_fwd_tc_kernel<MASK><<<grid, kThreads, sizeof(NeusTcSmem), (cudaStream_t)stream>>>(*g, points, (const __half2*)table_h, W1, b1, W2,
-                                                                                                  b2, radius, n_out, sdf, grad, feature, n, n_dev,
-                                                                                                  n_active);
+    attr_set = true;
   }
+  const int grid = (int)min((int64_t)nsr_sm_count() * 4, (n + kThreads - 1) / kThreads);
+  neus_field_fwd_tc_kernel<MASK><<<grid, kThreads, sizeof(NeusTcSmem), (cudaStream_t)stream>>>(*g, points, (const __half2*)table_h, W1, b1, W2, b2,
+                                                                                                radius, n_out, sdf, grad, feature, n, n_dev, n_active);
   NSR_CHECK_LAUNCH(name);
   return 0;
 }

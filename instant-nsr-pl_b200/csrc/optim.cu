@@ -6,7 +6,6 @@
 // parameter.  Arithmetic follows torch's single-tensor AdamW step by step (lerp for exp_avg, sqrt(v)/sqrt(bc2) + eps).
 #include "common.cuh"
 #include <math.h>
-#include <stdlib.h>
 
 namespace {
 
@@ -28,7 +27,8 @@ __device__ __forceinline__ void adam_one(float& p, float g, float& m, float& v, 
   p -= c.step_size * (m / denom);
 }
 
-// U float4 groups per thread per iteration (all loads issued before the first use), grid-stride over U * blockDim chunks.
+// U float4 groups per thread per iteration (all loads issued before the first use), grid-stride over U * blockDim chunks.  nsr_adamw_step
+// launches U = 1 with one CTA per chunk: U = 2 / 4 and grids capped at 8 or 16 CTAs per SM were not faster on the H100.
 template <int U>
 __global__ void __launch_bounds__(256) adamw_kernel(AdamConsts c, float* __restrict__ params, const float* __restrict__ grads,
                                                     float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
@@ -130,24 +130,8 @@ extern "C" int nsr_adamw_step(const nsr_adamw_t* h, float* params, const float* 
   c.inv_scale = h->inv_grad_scale;
   c.lr = h->lr;
   c.weight_decay = h->weight_decay;
-  // launch shape: NSR_ADAMW_VARIANT = "<unroll 1|2|4>,<ctas per SM, 0 = one CTA per chunk>" (development knob; tools/adamw_bench.py sweeps it)
-  static int unroll = 1, ctas_per_sm = 0;
-  static bool read_env = false;
-  if (!read_env) {
-    if (const char* e = getenv("NSR_ADAMW_VARIANT")) sscanf(e, "%d,%d", &unroll, &ctas_per_sm);
-    read_env = true;
-  }
-  const int64_t n4 = n >> 2;
-  const int u = unroll == 4 ? 4 : (unroll == 2 ? 2 : 1);
-  const int64_t chunks = max((int64_t)1, (n4 + 256 * u - 1) / (256 * u));
-  const int grid = (int)(ctas_per_sm > 0 ? min(chunks, (int64_t)nsr_sm_count() * ctas_per_sm) : chunks);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (u == 1)
-    adamw_kernel<1><<<grid, 256, 0, st>>>(c, params, grads, exp_avg, exp_avg_sq, (__half*)params_half, dev_lr_step, found_inf, n);
-  else if (u == 2)
-    adamw_kernel<2><<<grid, 256, 0, st>>>(c, params, grads, exp_avg, exp_avg_sq, (__half*)params_half, dev_lr_step, found_inf, n);
-  else
-    adamw_kernel<4><<<grid, 256, 0, st>>>(c, params, grads, exp_avg, exp_avg_sq, (__half*)params_half, dev_lr_step, found_inf, n);
+  const int grid = (int)max((int64_t)1, ((n >> 2) + 255) / 256);   // one CTA per 1024-float chunk
+  adamw_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(c, params, grads, exp_avg, exp_avg_sq, (__half*)params_half, dev_lr_step, found_inf, n);
   NSR_CHECK_LAUNCH("nsr_adamw_step");
   return 0;
 }

@@ -256,8 +256,7 @@ class NerfFused:
         self.mode = 'two_pass' if self.contracted else 'per_ray'
         self.lean_static_outputs = False   # static=True: skip the per-ray outputs the fused loss op produces itself (comp_rgb, rays_valid)
         self.packed_bwd_inputs = True   # tile backward reads its inputs in packed row order (written by nsr_pack_kept)
-        from .config import experimental
-        self.fuse_kept_scan = experimental('pack_scan')   # nsr_pack_kept_scan instead of nsr_scan_counts + nsr_pack_kept (not yet timed)
+        self.fuse_kept_scan = True   # nsr_pack_kept_scan instead of nsr_scan_counts + nsr_pack_kept
         # 'tiles_split' (default: network half + high-occupancy table scatter) | 'tiles' (one sample-tile backward kernel, REDs from the
         # MMA warps) | 'tc' (wgmma / TMA warp-specialised kernel: csrc/nerf_bwd_tc.cu) | 'rays' (single per-ray backward kernel)
         import os

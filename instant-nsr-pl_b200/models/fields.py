@@ -8,7 +8,6 @@ from . import register
 from ..nerfacc import ContractionType
 from .common import BaseModel, get_activation, scale_anything, update_module_step
 from .networks import get_encoding, get_mlp, get_encoding_with_network, VanillaMLP
-from ..config import experimental
 from .. import ops, tcnn
 
 
@@ -332,7 +331,7 @@ class VolumeRadiance(nn.Module):
         """VanillaMLP colour network (neus-dtu.yaml:58-70,93-105: ReLU, 64 x 2 hidden, biases) on the same one-kernel path
         (nsr_radiance_vanilla_*); input cat[feature | SH4 | extra] at most 32 wide."""
         net = self.network
-        if not self.config.get('fused_vanilla', experimental('radiance_vanilla')):
+        if not self.config.get('fused_vanilla', True):
             return None
         if net.sphere_init or net.n_neurons != 64 or net.n_hidden_layers != 2 or len(args) > 1 or features.dim() != 2 or dirs.dim() != 2:
             return None

@@ -112,17 +112,15 @@ class VanillaMLP(nn.Module):
                 mods.append(self.make_activation())
         self.layers = nn.Sequential(*mods)
         self.output_activation = get_activation(config['output_activation'])
-        # our extension key: True = fused kernel (nsr_mlp_vanilla_*), False = torch (cuBLAS) layers, absent = nsr_b200.config.experimental
-        self.fused = None if config.get('fused', None) is None else bool(config['fused'])
+        # our extension key: True (default) = fused kernel (nsr_mlp_vanilla_*), False = torch (cuBLAS) layers
+        self.fused = bool(config.get('fused', True))
         self._spec = None
 
     def _fused_spec(self, x):
         """VanillaMlpSpec when this network maps onto the one-kernel path (ReLU, 64 neurons, <= 3 hidden layers, n_in <= 64,
         n_out <= 16, CUDA input, no double backward needed => not the sphere-init SDF network); None -> torch layers."""
         from .. import ops
-        from ..config import experimental
-        want = experimental('mlp_vanilla') if self.fused is None else self.fused
-        if self.sphere_init or not x.is_cuda or not want or ops.static_rows_active():
+        if self.sphere_init or not x.is_cuda or not self.fused or ops.static_rows_active():
             return None
         if self._spec is None:
             lins = [m for m in self.layers if isinstance(m, nn.Linear)]

@@ -6,7 +6,6 @@ import sys, os, types, importlib.util, traceback
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT); sys.path.insert(0, ROOT+'/tests/helpers'); sys.path.insert(0, ROOT+'/tests')
-os.environ['NSR_EXPERIMENTAL']='1'
 import cpu_thirdparty as tp
 from nsr_b200 import models as ours, tcnn as our_tcnn, nerfacc as nacc
 from nsr_b200.models import nerf_model, neus_model

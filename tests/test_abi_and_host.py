@@ -164,20 +164,10 @@ def test_vanilla_mlp_packing_matches_layers_and_routes_gradients():
         ops.RadianceSpec(16, 3, 2, vanilla=True)
 
 
-def test_experimental_switch_and_vanilla_mlp_stays_on_torch_for_cpu(monkeypatch):
-    from nsr_b200.config import experimental
+def test_vanilla_mlp_is_fused_by_default_and_stays_on_torch_for_cpu():
     from nsr_b200.models.networks import VanillaMLP
-    monkeypatch.delenv('NSR_EXPERIMENTAL', raising=False)
-    monkeypatch.delenv('NSR_DISABLE', raising=False)
-    assert experimental('mlp_vanilla') and experimental('radiance_vanilla') and not experimental('something_new')   # validated paths: on
-    monkeypatch.setenv('NSR_DISABLE', 'mlp_vanilla, other')
-    assert not experimental('mlp_vanilla') and experimental('radiance_vanilla')
-    monkeypatch.delenv('NSR_DISABLE')
-    monkeypatch.setenv('NSR_EXPERIMENTAL', 'new_a, new_b')
-    assert experimental('new_a') and experimental('new_b') and not experimental('new_c')
-    monkeypatch.setenv('NSR_EXPERIMENTAL', '1')
-    assert experimental('anything')
     net = VanillaMLP(8, 3, dict(n_neurons=64, n_hidden_layers=2, output_activation='none'))
+    assert net.fused and not VanillaMLP(8, 3, dict(n_neurons=64, n_hidden_layers=2, output_activation='none', fused=False)).fused
     x = torch.randn(5, 8)
     assert net._fused_spec(x) is None and net(x).shape == (5, 3)   # CPU tensors: the torch layers (the reference's own CPU behaviour)
 

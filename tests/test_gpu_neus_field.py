@@ -1,4 +1,4 @@
-"""The fused NeuS SDF field kernels (nsr_neus_field_fwd, tensor-core and scalar forwards; nsr_neus_field_bwd, first- and second-order
+"""The fused NeuS SDF field kernels (nsr_neus_field_fwd, the tensor-core forward; nsr_neus_field_bwd, first- and second-order
 backward; nsr_absmax3) entry by entry against the fp64 reference of tests/helpers/neus_field_ref.py.
 
 Every output entry must sit within rtol * M + floor of the reference (M: the entry's linearised absolute mass; floor: fp16's subnormal
@@ -10,9 +10,6 @@ Run with -s to see the headroom (worst |error| / bound) per output.  The weight 
 with no rows to average over, an entry may be a full fp16 rounding of both tile operands (or half a subnormal step) from the reference,
 which is exactly what the bound allows."""
 import ctypes
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -28,7 +25,6 @@ GRID = dict(otype='HashGrid', n_levels=16, n_features_per_level=2, log2_hashmap_
 GRIDS = {'prod': GRID, 'small': dict(GRID, log2_hashmap_size=12)}
 C3_SAMPLES = 183584
 SENTINEL = 777.0
-SCALAR = os.environ.get('NSR_NEUS_FWD', '')[:1] == 's'
 HEADROOM = {}
 
 
@@ -74,7 +70,7 @@ def env():
     e = Env()
     yield e
     if HEADROOM:
-        print(f'\nworst |error| / (rtol M + floor) per output ({"scalar" if SCALAR else "tensor-core"} forward):')
+        print('\nworst |error| / (rtol M + floor) per output:')
         for k, v in sorted(HEADROOM.items()):
             print(f'  {k:34s} {v:.3f}')
 
@@ -153,7 +149,7 @@ def check(E, grid, inp, k, got, tag, parts=nr.FWD_PARTS + nr.BWD_PARTS, amax='ab
             g[p] = got[p][:k]
     head = nr.check_all(g, R, parts=parts, what=f'{tag} k={k}', prefill=prefill)
     for p, v in head.items():
-        name = f'{"scalar " if SCALAR and p in nr.FWD_PARTS else ""}{p} ({tag.split(" ")[0]})'
+        name = f'{p} ({tag.split(" ")[0]})'
         HEADROOM[name] = max(HEADROOM.get(name, 0.0), v)
     return R, head
 
@@ -172,7 +168,7 @@ def test_row_counts(env, idx):
 
 
 def test_forward_row_counts(env):
-    """every row count through the forward only (test_scalar_forward runs this with NSR_NEUS_FWD=scalar)"""
+    """every row count through the forward only"""
     inp = env.inputs()
     for k in env.ks():
         got = run(env, 'prod', inp, k, k + 77, bwd=False)
@@ -360,14 +356,3 @@ def test_absmax3(env):
     a2, b2, c2 = a[:k].contiguous(), b[:k].contiguous(), c[:k].contiguous()
     assert call(a2, b2, c2, None, k) == want
 
-
-def test_scalar_forward():
-    """the thread-per-sample fp32 forward (NSR_NEUS_FWD=scalar, read once per process) on the same row counts and bounds"""
-    here = os.path.dirname(os.path.abspath(__file__))
-    env_vars = dict(os.environ, NSR_NEUS_FWD='scalar')
-    cmd = [sys.executable, '-m', 'pytest', '-q', '-s', '-p', 'no:cacheprovider', os.path.join(here, 'test_gpu_neus_field.py'), '-k',
-           'test_forward_row_counts']
-    p = subprocess.run(cmd, env=env_vars, capture_output=True, text=True, timeout=600, cwd=os.path.dirname(here))
-    lines = [l for l in p.stdout.splitlines() if 'scalar' in l or 'passed' in l or 'failed' in l]
-    print('\n' + '\n'.join(lines))
-    assert p.returncode == 0, p.stdout[-4000:] + p.stderr[-2000:]

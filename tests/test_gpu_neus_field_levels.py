@@ -6,9 +6,6 @@ slices.  That is exact: a zero table gives zero features and a zero Jacobian on 
 run on the real table, whose masked levels hold random nonzero values, so every check also shows that those levels are ignored: their
 grad_table slices are left bit for bit as they were, and the dW1 columns of their features receive exactly 0."""
 import ctypes
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -22,7 +19,6 @@ D = 'cuda'
 GRID = dict(otype='HashGrid', n_levels=16, n_features_per_level=2, log2_hashmap_size=19, base_resolution=32,
             per_level_scale=1.3195079107728942)
 SENTINEL = 777.0
-SCALAR = os.environ.get('NSR_NEUS_FWD', '')[:1] == 's'
 LEVELS = (0, 1, 4, 9, 15, 16)
 
 
@@ -171,7 +167,7 @@ def test_levels(env, n_active):
 
 
 def test_forward_levels(env):
-    """the forward alone at every level count (test_scalar_forward runs it on the thread-per-sample kernel)"""
+    """the forward alone at every level count"""
     k = 128 * env.S + 33
     inp = env.inputs(k, seed=3)
     for n_active in LEVELS:
@@ -269,12 +265,3 @@ def test_graph_replay_follows_the_level_word(env):
     assert torch.equal(got['table'][single], eager['table'][single])
     check(env, got, R, k, 5, 'graph@5')
 
-
-def test_scalar_forward():
-    """the thread-per-sample forward (NSR_NEUS_FWD=scalar, read once per process) under the mask: the same checks in a subprocess"""
-    here = os.path.dirname(os.path.abspath(__file__))
-    env_vars = dict(os.environ, NSR_NEUS_FWD='scalar')
-    cmd = [sys.executable, '-m', 'pytest', '-q', '-p', 'no:cacheprovider', os.path.join(here, 'test_gpu_neus_field_levels.py'), '-k',
-           'test_forward_levels or test_sixteen_levels']
-    p = subprocess.run(cmd, env=env_vars, capture_output=True, text=True, timeout=600, cwd=os.path.dirname(here))
-    assert p.returncode == 0 and '2 passed' in p.stdout, p.stdout[-4000:] + p.stderr[-2000:]

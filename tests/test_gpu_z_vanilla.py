@@ -17,7 +17,7 @@ pre-activation that sits within ~5e-4 of zero for about one hidden unit in a tho
 its whole contribution, which is why the check is a quantile and not a max-abs bound.  The same effect exists
 between tiny-cuda-nn's fp16 FullyFusedMLP and an fp32 torch MLP in the reference.
 
-The kernels are the default for the VanillaMLP colour / background networks (nsr_b200.config.VALIDATED)."""
+The kernels are the default for the VanillaMLP colour / background networks (config keys fused / fused_vanilla, default true)."""
 import os
 
 import pytest
