@@ -423,6 +423,19 @@ int nsr_neus_composite_bwd(const float* alphas, const float* rgbs, const float* 
                            const float* weights, const float* trans, const int64_t* offsets, const float* g_weights,
                            const float* g_opacity, const float* g_depth, const float* g_rgb, const float* g_normal, float* d_alphas,
                            float* d_rgbs, float* d_normals, int64_t n_rays, void* stream);
+/* nsr_neus_render_rays: NeuSModel.forward_ in eval mode (models/neus.py:205-243, randomized = False) for a pass of rays in ONE kernel:
+ * a warp owns a ray (ticket: device uint32, zero on entry, over the longest-first queue of nsr_march_rays_alloc: masks / words / t_min /
+ * counts / bin_counts / order_bins as that function wrote them), walks its marched samples in groups of 32 consecutive samples (the
+ * groups of nsr_neus_composite_fwd) and runs sample points, the SDF field with its analytic normal (weights as nsr_neus_field_fwd_levels;
+ * n_active: device float, 16 for a plain HashGrid), alpha (inv_s, cos_anneal: device scalars, as nsr_neus_alpha_fwd), the colour network
+ * (rp: n_feat 13, n_extra 3 = the unit normal; vanilla 0: FullyFused as nsr_radiance_fwd, 1: VanillaMLP as nsr_radiance_vanilla_fwd with
+ * rgb_bias) and the compositing in registers.  Writes per ray only: opacity [n,1], depth [n,1], comp_rgb [n,3] (before the background),
+ * comp_normal [n,3] (un-normalised); every marched sample is composited (no transmittance cut-off). */
+int nsr_neus_render_rays(const nsr_grid_t* g, const float* rays, const uint32_t* masks, int32_t words, const float* t_min, const int32_t* counts,
+                         const int32_t* bin_counts, const int32_t* order_bins, float step, const void* table_h, const float* W1, const float* b1,
+                         const float* W2, const float* b2, float radius, int32_t n_out, const float* n_active, const nsr_radiance_t* rp,
+                         int32_t vanilla, const void* rgb_params_h, const float* rgb_bias, const float* inv_s, const float* cos_anneal,
+                         float* opacity, float* depth, float* comp_rgb, float* comp_normal, uint32_t* ticket, int64_t n_rays, void* stream);
 /* VolumeRadiance (see nsr_radiance_t): feat f32 [n,n_feat], dirs f32 [n,3] (unit view directions, per sample), extra f32 [n,n_extra] (or NULL), params fp16 [7168] in tcnn order,
  * rgb f32 [n,3].  Backward: d_rgb [n,3] -> d_feat, d_extra (either may be NULL), grad_params f32 [7168] (+=);
  * loss_scale <= 0: choose the fp16 dgrad scale from *amax (device float: max |d_rgb|). */

@@ -10,7 +10,7 @@
 // ray, 32 lattice points per iteration, ballot + popc compaction -- against a packed BITfield
 // (128^3 bits = 256 KB, L1/L2 resident; nerfacc reads 2 MB of bools).  Two passes (count, write)
 // around a device-side exclusive scan keep nerfacc's exact-size, ray-ordered output contract.
-#include "common.cuh"
+#include "march.cuh"
 
 namespace {
 
@@ -280,8 +280,8 @@ __global__ void __launch_bounds__(kMarchWarps * 32) march_rays_expand_kernel(nsr
       const float k = (float)(w * 32 + b);
       if (pos < end) {
         ray_indices[pos] = (int32_t)ray;
-        t_starts[pos] = __fmaf_rn(k, step, tmin);
-        t_ends[pos] = __fmaf_rn(k + 1.f, step, tmin);
+        t_starts[pos] = nsr_lattice_t(k, step, tmin);
+        t_ends[pos] = nsr_lattice_t(k + 1.f, step, tmin);
       }
       ++pos;
     }
@@ -526,11 +526,11 @@ __global__ void __launch_bounds__(256) sample_points_kernel(const float* __restr
   if (i >= n) return;
   const float* r = rays + (size_t)ray_indices[i] * 6;
   const float t0 = t_starts[i], t1 = t_ends[i];
-  const float mid = (t0 + t1) / 2.f;
+  const float mid = nsr_sample_mid(t0, t1);
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     const float d = __ldg(r + 3 + c);
-    positions[i * 3 + c] = __ldg(r + c) + d * mid;
+    positions[i * 3 + c] = nsr_sample_coord(__ldg(r + c), d, mid);
     if (dirs) dirs[i * 3 + c] = d;
   }
   if (dists) dists[i] = t1 - t0;

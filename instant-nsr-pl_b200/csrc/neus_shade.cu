@@ -6,35 +6,9 @@
 //   iter_cos  = -(relu(-true_cos/2 + 1/2) (1 - a) + relu(-true_cos) a)          a = cos_anneal_ratio
 //   prev/next = sdf -/+ iter_cos * dist / 2
 //   alpha     = clip((sigmoid(s prev) - sigmoid(s next) + 1e-5) / (sigmoid(s prev) + 1e-5), 0, 1)      s = inv_s (device scalar)
-#include "common.cuh"
+#include "neus_shade.cuh"
 
 namespace {
-
-struct AlphaTerms {
-  float nx, ny, nz, inv_norm, true_cos, iter_cos, dist, prev, next, pc, nc, q;
-};
-
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
-
-__device__ __forceinline__ AlphaTerms alpha_terms(float sdf, float gx, float gy, float gz, float dx, float dy, float dz, float dist, float s,
-                                                  float a) {
-  AlphaTerms t;
-  const float nrm = fmaxf(sqrtf(gx * gx + gy * gy + gz * gz), 1e-12f);
-  t.inv_norm = 1.f / nrm;
-  t.nx = gx * t.inv_norm;
-  t.ny = gy * t.inv_norm;
-  t.nz = gz * t.inv_norm;
-  t.true_cos = dx * t.nx + dy * t.ny + dz * t.nz;
-  t.iter_cos = -(fmaxf(-t.true_cos * 0.5f + 0.5f, 0.f) * (1.f - a) + fmaxf(-t.true_cos, 0.f) * a);
-  t.dist = dist;
-  const float h = t.iter_cos * dist * 0.5f;
-  t.prev = sdf - h;
-  t.next = sdf + h;
-  t.pc = sigmoidf_(t.prev * s);
-  t.nc = sigmoidf_(t.next * s);
-  t.q = (t.pc - t.nc + 1e-5f) / (t.pc + 1e-5f);
-  return t;
-}
 
 __global__ void __launch_bounds__(256) neus_alpha_fwd_kernel(const float* __restrict__ sdf, const float* __restrict__ sdf_grad,
                                                              const float* __restrict__ dirs, const float* __restrict__ dists,

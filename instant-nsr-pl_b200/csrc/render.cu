@@ -3,42 +3,11 @@
 // (models/nerf.py:87-92,105-109; models/neus.py:181-184,237-243).
 // One warp per ray walks the ray's contiguous sample segment in chunks of 32 with shuffle scans and a
 // running carry -- no CUB scan-by-key over the whole batch, no atomics, deterministic results.
-#include "common.cuh"
+#include "warp_scan.cuh"
 
 namespace {
 
 constexpr int kWarps = 8;
-
-__device__ __forceinline__ float warp_incl_sum(float v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += t;
-  }
-  return v;
-}
-__device__ __forceinline__ float warp_incl_prod(float v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v *= t;
-  }
-  return v;
-}
-// inclusive suffix sum (lane i gets sum over lanes >= i)
-__device__ __forceinline__ float warp_suffix_sum(float v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float t = __shfl_down_sync(0xffffffffu, v, o);
-    if (lane + o < 32) v += t;
-  }
-  return v;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 #define RAY_PROLOGUE                                                      \
   const int lane = threadIdx.x & 31;                                      \

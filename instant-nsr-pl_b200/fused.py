@@ -45,6 +45,7 @@ class _NerfRender(torch.autograd.Function):
         need_grad = any(p.requires_grad for p in params)
         enc = torch.empty(cap, 32, dtype=torch.float16, device=dev) if need_grad else None
         k_dev = st['offsets_k'][n_rays:]
+        fused.last_offsets_k = st['offsets_k']   # per-ray kept counts of the last render (NeuS eval: num_samples_bg per slice)
         fused.render_fwd(kp, rays, st['ri'], st['ts'], st['te'], st['trans'], enc, sig, rgbs, weights, acc_rgb, opacity, depth, cap, k_dev)
         ctx.fused, ctx.n_rays, ctx.cap, ctx.n_kp = fused, n_rays, cap, len(kp)
         ctx.set_materialize_grads(False)

@@ -144,6 +144,20 @@ class VolumeSDF(BaseImplicitGeometry):
         except AttributeError:
             return False
 
+    def fused_render_unsupported(self):
+        """None when NeuS eval rendering can run this field inside the per-ray kernel (ops.neus_render_rays: the fused analytic
+        field with a 13-wide output), else why it keeps the per-sample path (a message)."""
+        if self.grad_type != 'analytic':
+            return 'finite-difference normals (neuralangelo) evaluate a seven-point stencil per sample: per-sample eval path'
+        if self._progressive and not self.config.get('fused_progressive', False):
+            return 'a ProgressiveBandHashGrid runs the fused field only with fused_progressive: true'
+        if not self._fused:
+            return ('the geometry is not the fused SDF field shape (include_xyz HashGrid L=16 F=2 + sphere-init VanillaMLP 35 -> 64 -> n_out, '
+                    'analytic normals)')
+        if self.n_output_dims != 13:
+            return f'the colour input is [feature 13 | SH4 | normal]: feature_dim is {self.n_output_dims}'
+        return None
+
     def _n_active_levels(self):
         return int(self.encoding.encoding.current_level) if self._progressive else 16
 

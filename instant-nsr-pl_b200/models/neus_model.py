@@ -73,6 +73,35 @@ def _logistic_alpha(prev_sdf, next_sdf, inv_s):
     return ((prev_cdf - next_cdf + 1e-5) / (prev_cdf + 1e-5)).clip(0.0, 1.0)
 
 
+def slice_sums(per_ray, ray_chunk):
+    """chunk_batch's num_samples layout: one int32 entry per ``ray_chunk`` slice of the rays, the per-ray counts summed per slice."""
+    pad = (-per_ray.shape[0]) % ray_chunk
+    return F.pad(per_ray.to(torch.int64), (0, pad)).view(-1, ray_chunk).sum(1).to(torch.int32)
+
+
+def fused_eval_dict(fg, ray_chunk, background_color=None, bg=None):
+    """The eval-mode dict of ``chunk_batch(forward_, ray_chunk, True, rays)`` (same keys, dtypes, shapes, on the CPU) from per-ray
+    tensors: fg = dict(opacity [N,1], depth [N,1], comp_rgb [N,3] before the background, comp_normal [N,3] un-normalised, counts [N]);
+    bg = None (constant ``background_color``) or the learned background's dict(comp_rgb [N,3] blended, opacity, depth, counts)."""
+    opacity, comp_rgb = fg['opacity'], fg['comp_rgb']
+    valid = opacity > 0
+    num = slice_sums(fg['counts'], ray_chunk)
+    out = {'comp_rgb': comp_rgb, 'comp_normal': F.normalize(fg['comp_normal'], p=2, dim=-1), 'opacity': opacity, 'depth': fg['depth'],
+           'rays_valid': valid, 'num_samples': num}
+    if bg is None:
+        out_bg = {'comp_rgb': background_color[None, :].expand(*comp_rgb.shape), 'num_samples': torch.zeros_like(num),
+                  'rays_valid': torch.zeros_like(valid)}
+    else:
+        out_bg = {'comp_rgb': bg['comp_rgb'], 'opacity': bg['opacity'], 'depth': bg['depth'], 'rays_valid': bg['opacity'] > 0,
+                  'num_samples': slice_sums(bg['counts'], ray_chunk)}
+    out_full = {'comp_rgb': comp_rgb + out_bg['comp_rgb'] * (1.0 - opacity), 'num_samples': num + out_bg['num_samples'],
+                'rays_valid': valid | out_bg['rays_valid']}
+    merged = dict(out)
+    merged.update({k + '_bg': v for k, v in out_bg.items()})
+    merged.update({k + '_full': v for k, v in out_full.items()})
+    return {k: v.contiguous().cpu() for k, v in merged.items()}
+
+
 @register('neus')
 class NeuSModel(BaseModel):
     def setup(self):
@@ -318,8 +347,81 @@ class NeuSModel(BaseModel):
         merged.update({k + '_full': v for k, v in out_full.items()})
         return merged
 
+    def fused_render_unsupported(self):
+        """None when eval-mode forward() renders through the per-ray kernel (ops.neus_render_rays; model config key
+        ``fused_render: true``), else why it keeps the per-sample path of chunk_batch(forward_) (a message)."""
+        cfg = self.config
+        if not cfg.get('fused_render', False):
+            return 'fused_render is off'
+        if not cfg.grid_prune:
+            return 'the per-ray renderer marches the occupancy grid: needs grid_prune'
+        why = self.geometry.fused_render_unsupported()
+        if why is not None:
+            return why
+        if cfg.learned_background:
+            from ..fused import NerfBackgroundFused
+            missing = NerfBackgroundFused.unsupported(self)
+            if missing is not None:
+                return f'the learned background needs {missing}'
+        return None
+
+    def _render_spec(self, dev):
+        """the colour network's RadianceSpec for [feature 13 | SH4 | normal] rows, or None when it is not the fused shape"""
+        n_feat = self.geometry.n_output_dims
+        e = lambda k: torch.empty(0, k, device=dev)
+        return self.texture._fused_spec(e(n_feat), e(3), (e(3),))
+
+    @torch.no_grad()
+    def _render_fused(self, rays):
+        """eval-mode forward() on the per-ray kernel: passes of config.render_chunk rays, outputs kept on the device and copied to
+        the CPU once; the learned background runs its sync-free executor (NerfBackgroundFused.render(static=True)) per pass."""
+        import math
+        cfg, geo, tex = self.config, self.geometry, self.texture
+        rays = rays.float().contiguous()
+        dev = rays.device
+        spec = self._render_spec(dev)
+        grid = self.occupancy_grid
+        if self._march_static is None:
+            r = float(cfg.radius)
+            self._march_static = (ops.march_struct(grid.roi_host(), grid._res, ContractionType.AABB.value, self.render_step_size, 0.0),
+                                  int(math.ceil(2.0 * math.sqrt(3.0) * r / self.render_step_size)) + 2)
+        ms, cap_per_ray = self._march_static
+        if self._cos_dev is None or self._cos_dev.device != dev:
+            self._cos_dev = torch.full((1,), float(self.cos_anneal_ratio), device=dev)
+        enc = geo._fd_grid()
+        W1, b1, W2, b2 = geo._effective_weights()
+        n_active = geo._fd_state[2:] if geo._progressive else torch.full((1,), 16.0, device=dev)
+        inv_s = self.variance.inv_s.clip(1e-6, 1e6).reshape(1)
+        if spec.vanilla:
+            weights, rgb_bias = ops.pack_vanilla_radiance(tex.network.linear_params())
+            rgb_params = weights.to(torch.float16)
+        else:
+            rgb_params, rgb_bias = tex.network._params_half(), None
+        bg_fused = self._static_background() if cfg.learned_background else None
+        chunk = int(cfg.get('render_chunk', 65536))
+        fg, bg, overflow = [], [], []
+        for s in range(0, rays.shape[0], chunk):
+            r = rays[s:s + chunk]
+            fg.append(ops.neus_render_rays(ms, r, grid.bits(), grid.coarse_bits(), cap_per_ray, enc.grid, geo.radius, enc._params_half(), W1, b1,
+                                           W2, b2, n_active, spec, rgb_params, rgb_bias, inv_s, self._cos_dev))
+            if bg_fused is not None:
+                o = bg_fused.render(r, None, static=True)
+                off = bg_fused.last_offsets_k
+                bg.append({'comp_rgb': o['comp_rgb'], 'opacity': o['opacity'], 'depth': o['depth'], 'counts': off[1:] - off[:-1]})
+                overflow.append(o['overflow'])
+        cat = lambda parts: {k: torch.cat([p[k] for p in parts]) for k in parts[0]}
+        out = fused_eval_dict(cat(fg), cfg.ray_chunk, self.background_color, cat(bg) if bg else None)
+        if overflow:
+            assert not bool(torch.cat(overflow).any()), 'learned background: samples past the static capacity were dropped'
+        return out
+
     def forward(self, rays):
-        out = self.forward_(rays) if self.training else chunk_batch(self.forward_, self.config.ray_chunk, True, rays)
+        if self.training:
+            out = self.forward_(rays)
+        elif rays.is_cuda and rays.shape[0] > 0 and self.fused_render_unsupported() is None and self._render_spec(rays.device) is not None:
+            out = self._render_fused(rays)
+        else:
+            out = chunk_batch(self.forward_, self.config.ray_chunk, True, rays)
         return {**out, 'inv_s': self.variance.inv_s}
 
     def train(self, mode=True):
