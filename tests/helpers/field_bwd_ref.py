@@ -102,32 +102,48 @@ def _act_perturbation(pre, live, tie, bnd, acc):
     return flip + torch.where(tie, pre.abs() + bnd, torch.zeros_like(pre))
 
 
+def relu_ties(act_in, p_in, layers, acc_rel=ACC_REL, second_order=False):
+    """ReLU decisions the kernel may take the other way, for a chain of fp16 ReLU layers.  act_in: the chain's fp16 input (its
+    absolute value is the accumulation mass), p_in: how far the kernel's input can be from it; layers: [(pre-activation, weight
+    [out, in], fp32 bias or None, fp16 post-activation)].  The bound on |kernel pre - our pre| is the fp32 accumulation error of the
+    absolute mass (bias included) plus the input perturbation through |W|.  Returns the tie masks per layer and the perturbation of
+    the last post-activation.
+    second_order: wherever the whole bound (accumulation error plus upstream perturbation) reaches a rounding midpoint, a live
+    activation may be off by that bound plus one ulp (rounding two values |a - b| <= bnd apart lands at most |a - b| + ulp apart,
+    and on the same value when no midpoint lies between them) -- what a check that is exact outside the predicted flips needs.
+    Without it, _act_perturbation's first-order rule: enough where rtol absorbs one-ulp flips."""
+    ties, act_in = [], act_in.double().abs()
+    for pre, Wm, b, post in layers:
+        Wa = Wm.double().abs()
+        pre = pre.double()
+        acc = acc_rel * (act_in @ Wa.T + (0.0 if b is None else b.double().abs()))
+        prop = p_in.double() @ Wa.T
+        bnd = acc + prop
+        tie = (pre.abs() <= bnd) & (bnd > 0)   # (no mass: every term is an exact zero, on the device too)
+        if second_order:
+            zero = torch.zeros_like(pre)
+            p_in = (torch.where(((post > 0) | tie) & (_mid_dist(pre) <= bnd), _ulp16(pre) + bnd, zero)
+                    + torch.where(tie, pre.abs() + bnd, zero))
+        else:
+            p_in = _act_perturbation(pre, post > 0, tie, bnd, acc)
+        act_in = post.double().abs()
+        ties.append(tie)
+    return ties, p_in
+
+
 def _tie_masks(A, W):
     """per pre-activation: can the kernel's ReLU decision differ from ours?  The bound on |kernel pre - our pre| is the fp32
     accumulation error plus the fp16 rounding flips it allows upstream, propagated layer by layer."""
-    Wa = {k: v.double().abs() for k, v in W.items()}
-    E = A['E'].double().abs()
-    mass = E @ Wa['DW1'].T
-    bnd = ACC_REL * mass
-    h1 = A['pre']['h1'].double()
-    tie_h1 = (h1.abs() <= bnd) & (bnd > 0)   # (no mass: every term is an exact zero, on the device too)
-    p_h1 = _act_perturbation(h1, A['H1'] > 0, tie_h1, bnd, bnd)
+    E = A['E'].double()
+    (tie_h1,), _ = relu_ties(E, torch.zeros_like(E), [(A['pre']['h1'], W['DW1'], None, A['H1'])])
     H1 = A['H1'].double()
     o = H1 @ W['DW2'].double().T
-    p_o = _ulp16(o) * (_mid_dist(o) <= ACC_REL * (H1 @ Wa['DW2'].T))
+    p_o = _ulp16(o) * (_mid_dist(o) <= ACC_REL * (H1 @ W['DW2'].double().abs().T))
     sh = A['sh32'].double()
     p_sh = _ulp16(sh) * (_mid_dist(sh) <= SH_ABS)
-    p_ci = torch.cat([p_o, p_sh], 1)
-    ties, p_in, act_in = [tie_h1], p_ci, A['CI'].double().abs()
-    for key, wk, act in (('g1', 'CW1', 'G1'), ('g2', 'CW2', 'G2')):
-        pre = A['pre'][key].double()
-        acc = ACC_REL * (act_in @ Wa[wk].T)
-        bnd = acc + p_in @ Wa[wk].T
-        tie = (pre.abs() <= bnd) & (bnd > 0)
-        p_in = _act_perturbation(pre, A[act] > 0, tie, bnd, acc)
-        act_in = A[act].double()
-        ties.append(tie)
-    return ties
+    ties, _ = relu_ties(A['CI'], torch.cat([p_o, p_sh], 1),
+                        [(A['pre']['g1'], W['CW1'], None, A['G1']), (A['pre']['g2'], W['CW2'], None, A['G2'])])
+    return [tie_h1] + ties
 
 
 def backward(W, A, masks, dc3, dsr, ls, dtype, store=None, inject=0.0):
