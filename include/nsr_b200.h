@@ -436,6 +436,16 @@ int nsr_neus_render_rays(const nsr_grid_t* g, const float* rays, const uint32_t*
                          const float* W2, const float* b2, float radius, int32_t n_out, const float* n_active, const nsr_radiance_t* rp,
                          int32_t vanilla, const void* rgb_params_h, const float* rgb_bias, const float* inv_s, const float* cos_anneal,
                          float* opacity, float* depth, float* comp_rgb, float* comp_normal, uint32_t* ticket, int64_t n_rays, void* stream);
+/* nsr_neus_render_rays_fd: the same render with the finite-difference SDF field of nsr_neus_field_fd_fwd (Neuralangelo: W1 [64,35], b1,
+ * W2 [13,64], b2 as that function takes them).  fd_state (device {eps, eps^2, n_active}, non-NULL) replaces n_active.  Per sample,
+ * sdf and feature are the stencil centre's and the normal is the central difference 0.5 (s+ - s-) / eps in world units, with
+ * nsr_neus_field_fd_fwd's fp32 arithmetic and operation order: the per-sample path's values. */
+int nsr_neus_render_rays_fd(const nsr_grid_t* g, const float* rays, const uint32_t* masks, int32_t words, const float* t_min,
+                            const int32_t* counts, const int32_t* bin_counts, const int32_t* order_bins, float step, const void* table_h,
+                            const float* W1, const float* b1, const float* W2, const float* b2, float radius, int32_t n_out,
+                            const float* fd_state, const nsr_radiance_t* rp, int32_t vanilla, const void* rgb_params_h, const float* rgb_bias,
+                            const float* inv_s, const float* cos_anneal, float* opacity, float* depth, float* comp_rgb, float* comp_normal,
+                            uint32_t* ticket, int64_t n_rays, void* stream);
 /* VolumeRadiance (see nsr_radiance_t): feat f32 [n,n_feat], dirs f32 [n,3] (unit view directions, per sample), extra f32 [n,n_extra] (or NULL), params fp16 [7168] in tcnn order,
  * rgb f32 [n,3].  Backward: d_rgb [n,3] -> d_feat, d_extra (either may be NULL), grad_params f32 [7168] (+=);
  * loss_scale <= 0: choose the fp16 dgrad scale from *amax (device float: max |d_rgb|). */

@@ -3,11 +3,16 @@
 //   sample points -> SDF field + analytic normal (neus_field.cuh) -> alpha + unit normal (neus_shade.cuh) -> colour network
 //   [feature | SH4(dir) | normal] (radiance.cuh) -> transmittance scan with the carry in a register and per-lane sums (warp_scan.cuh)
 // and writes only per-ray results.  Nothing per sample reaches global memory.
+// The finite-difference form (FD, Neuralangelo's geometry) replaces only the field stage: each lane runs its own sample's centre
+// evaluation with every output and then the six stencil points for the SDF alone (neus_field_fd.cuh, fp32 on the CUDA cores, the
+// operation order of neus_fd_fwd_kernel), so sdf, feature and normal are the per-sample path's values; the normal is the world-space
+// central difference 0.5 (s+ - s-) / eps.
 // The groups are 32 CONSECUTIVE samples of the ray counted from its first, the groups neus_composite_fwd_kernel scans, so the
 // transmittance products and sums run in the same order as the per-sample path; samples and t come from march.cuh, so they are the
 // marcher's bit for bit.  Every marched sample is composited (the reference's NeuS has no transmittance cut-off).
 #include "march.cuh"
 #include "neus_field.cuh"
+#include "neus_field_fd.cuh"
 #include "neus_shade.cuh"
 #include "radiance.cuh"
 #include "warp_scan.cuh"
@@ -24,8 +29,16 @@ struct RenderWarpSmem {
   float rgb[32][4];
   float sh[16];            // SH4 of the ray's view direction: the same for every sample of the ray
 };
-constexpr size_t kRenderSmem = sizeof(NeusTcSmem) + W_TOTAL * sizeof(__half) + N_BIAS * sizeof(float) + kNeusTcWarps * sizeof(RenderWarpSmem);
-static_assert(sizeof(NeusTcSmem) % 16 == 0 && (W_TOTAL * sizeof(__half)) % 16 == 0 && (N_BIAS * sizeof(float)) % 16 == 0, "16-byte aligned");
+// shared memory: the field's weights (NeusTcSmem, or fd::FdW for the finite-difference form), the colour network, its bias, the warps' rows
+template <bool FD>
+constexpr size_t kFieldSmem = FD ? sizeof(fd::FdW) : sizeof(NeusTcSmem);
+template <bool FD>
+constexpr size_t kRenderSmem = kFieldSmem<FD> + W_TOTAL * sizeof(__half) + N_BIAS * sizeof(float) + kNeusTcWarps * sizeof(RenderWarpSmem);
+static_assert(sizeof(NeusTcSmem) % 16 == 0 && sizeof(fd::FdW) % 16 == 0 && (W_TOTAL * sizeof(__half)) % 16 == 0 &&
+                  (N_BIAS * sizeof(float)) % 16 == 0, "16-byte aligned");
+// CTAs per SM: the analytic form's 168 registers allow two; the finite-difference form's fit in 128 (four CTAs, 16 warps per SM)
+template <bool FD>
+constexpr int kCtasPerSm = FD ? 4 : 2;
 
 struct RenderArgs {
   const float* rays;            // [n, 6]
@@ -46,6 +59,7 @@ struct RenderArgs {
   float step, radius;
   int32_t words, n_out, act_mode;
   int64_t n_rays;
+  const float* fd_state;        // finite-difference form: {eps, eps^2, n_active} (n_active above is unused)
 };
 
 // the next (up to) 32 set bits of the ray's mask: lane j gets lattice index k of the j-th, or -1.  (cur_w, cur_m) is the warp-uniform
@@ -73,21 +87,28 @@ __device__ __forceinline__ int next_group(int lane, int words, uint32_t mw0, uin
 // The hash levels >= n_active (device float: the ProgressiveBandHashGrid schedule, 16 for a plain HashGrid) contribute 0, as in
 // neus_field_fwd_tc_kernel<true>; with n_active = 16 that is the unmasked field's arithmetic.  One masked form only: the unmasked
 // instantiation let the compiler hoist all sixteen levels' corner loads and spill.
-template <bool VANILLA>
-__global__ void __launch_bounds__(kThreads, 2) neus_render_rays_kernel(const __grid_constant__ nsr_grid_t g, const __grid_constant__ RenderArgs a) {
+// FD: the finite-difference field; eps and n_active come from fd_state, as in neus_fd_fwd_kernel.
+template <bool VANILLA, bool FD>
+__global__ void __launch_bounds__(kThreads, kCtasPerSm<FD>) neus_render_rays_kernel(const __grid_constant__ nsr_grid_t g,
+                                                                                    const __grid_constant__ RenderArgs a) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   NeusTcSmem& S = *reinterpret_cast<NeusTcSmem*>(smem_raw);
-  __half* RW = reinterpret_cast<__half*>(smem_raw + sizeof(NeusTcSmem));
+  fd::FdW& Wf = *reinterpret_cast<fd::FdW*>(smem_raw);
+  __half* RW = reinterpret_cast<__half*>(smem_raw + kFieldSmem<FD>);
   float* rbias = reinterpret_cast<float*>(RW + W_TOTAL);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   RenderWarpSmem& Wp = reinterpret_cast<RenderWarpSmem*>(rbias + N_BIAS)[warp];
   __shared__ int bins[NSR_ORDER_BINS];
-  stage_neus_tc_weights(S, a.W1, a.b1, a.W2, a.b2, a.n_out);
+  if constexpr (FD)
+    fd::stage_weights(Wf, a.W1, a.b1, a.W2, a.b2, a.n_out);
+  else
+    stage_neus_tc_weights(S, a.W1, a.b1, a.W2, a.b2, a.n_out);
   stage_weights(RW, a.rgb_params);
   if (VANILLA) stage_bias(rbias, a.rgb_bias);
   if (tid < NSR_ORDER_BINS) bins[tid] = __ldg(a.bin_counts + tid);
   __syncthreads();
-  const int n_active = load_n_active(a.n_active);
+  const int n_active = FD ? (int)__ldg(a.fd_state + 2) : load_n_active(a.n_active);
+  const float eps = FD ? __ldg(a.fd_state) : 0.f;
   const float inv_s = __ldg(a.inv_s), cos_anneal = __ldg(a.cos_anneal);
   const float inv2r = 1.f / (2.f * a.radius);
 
@@ -130,21 +151,54 @@ __global__ void __launch_bounds__(kThreads, 2) neus_render_rays_kernel(const __g
         if (!ok) k = 0;
         const float t0 = nsr_lattice_t((float)k, a.step, tmin), t1 = nsr_lattice_t((float)k + 1.f, a.step, tmin);
         const float mid = nsr_sample_mid(t0, t1);
-        float x = 0.5f, y = 0.5f, z = 0.5f;
-        if (ok) {   // neus_field_fwd_tc_kernel's unit-cube position of the sample point
-          x = (nsr_sample_coord(ox, dx, mid) + a.radius) * inv2r;
-          y = (nsr_sample_coord(oy, dy, mid) + a.radius) * inv2r;
-          z = (nsr_sample_coord(oz, dz, mid) + a.radius) * inv2r;
-        }
         float gx = 0.f, gy = 0.f, gz = 0.f;
-        neus_field_rows32<true>(
-            S, warp, lane, g, a.table, x, y, z, ok, n_active,
-            [&](int r0, int gq, int dr, int col, float v) { Wp.out[r0 + gq + dr][col] = v; },
-            [&](float gx_, float gy_, float gz_) {
-              gx = gx_ * inv2r;
-              gy = gy_ * inv2r;
-              gz = gz_ * inv2r;
-            });
+        if constexpr (FD) {
+          float px = 0.f, py = 0.f, pz = 0.f;   // world-space sample point (dead lanes: the box centre)
+          if (ok) {
+            px = nsr_sample_coord(ox, dx, mid);
+            py = nsr_sample_coord(oy, dy, mid);
+            pz = nsr_sample_coord(oz, dz, mid);
+          }
+          {  // centre: sdf and feature
+            float x, y, z, e[fd::NINP], out[fd::NOUTP];
+            fd::stencil_query(px, py, pz, 0, eps, a.radius, x, y, z);
+            fd::encode(g, a.table, x, y, z, n_active, e);
+            fd::mlp_eval<fd::NOUTP>(Wf, e, out);
+#pragma unroll
+            for (int c = 0; c < fd::NOUTP; ++c) Wp.out[lane][c] = out[c];
+          }
+          float sp = 0.f;   // SDF at the + point of the current axis
+#pragma unroll 1
+          for (int q = 1; q <= 6; ++q) {   // stencil points +x, -x, +y, -y, +z, -z: SDF only
+            float x, y, z, e[fd::NINP], sq[1];
+            fd::stencil_query(px, py, pz, q, eps, a.radius, x, y, z);
+            fd::encode(g, a.table, x, y, z, n_active, e);
+            fd::mlp_eval<1>(Wf, e, sq);
+            if (q & 1) {
+              sp = sq[0];
+            } else {
+              const float ga = __fdiv_rn(0.5f * (sp - sq[0]), eps);
+              gx = q == 2 ? ga : gx;
+              gy = q == 4 ? ga : gy;
+              gz = q == 6 ? ga : gz;
+            }
+          }
+        } else {
+          float x = 0.5f, y = 0.5f, z = 0.5f;
+          if (ok) {   // neus_field_fwd_tc_kernel's unit-cube position of the sample point
+            x = (nsr_sample_coord(ox, dx, mid) + a.radius) * inv2r;
+            y = (nsr_sample_coord(oy, dy, mid) + a.radius) * inv2r;
+            z = (nsr_sample_coord(oz, dz, mid) + a.radius) * inv2r;
+          }
+          neus_field_rows32<true>(
+              S, warp, lane, g, a.table, x, y, z, ok, n_active,
+              [&](int r0, int gq, int dr, int col, float v) { Wp.out[r0 + gq + dr][col] = v; },
+              [&](float gx_, float gy_, float gz_) {
+                gx = gx_ * inv2r;
+                gy = gy_ * inv2r;
+                gz = gz_ * inv2r;
+              });
+        }
         __syncwarp();
         const AlphaTerms at = alpha_terms(Wp.out[lane][0], gx, gy, gz, dx, dy, dz, t1 - t0, inv_s, cos_anneal);
         const float alpha = ok ? fminf(fmaxf(at.q, 0.f), 1.f) : 0.f;
@@ -203,21 +257,53 @@ __global__ void __launch_bounds__(kThreads, 2) neus_render_rays_kernel(const __g
   }
 }
 
-template <bool VANILLA>
-int launch(const nsr_grid_t* g, const RenderArgs& a, cudaStream_t st) {
+template <bool VANILLA, bool FD>
+int launch(const nsr_grid_t* g, const RenderArgs& a, cudaStream_t st, const char* name) {
   static thread_local bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(neus_render_rays_kernel<VANILLA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRenderSmem);
+    cudaError_t e = cudaFuncSetAttribute(neus_render_rays_kernel<VANILLA, FD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRenderSmem<FD>);
     if (e != cudaSuccess) {
-      nsr_set_error("nsr_neus_render_rays: cannot reserve %zu B shared memory: %s", kRenderSmem, cudaGetErrorString(e));
+      nsr_set_error("%s: cannot reserve %zu B shared memory: %s", name, kRenderSmem<FD>, cudaGetErrorString(e));
       return 2;
     }
     attr_set = true;
   }
-  const int grid = (int)min((int64_t)nsr_sm_count() * 2, (a.n_rays + kNeusTcWarps - 1) / kNeusTcWarps);
-  neus_render_rays_kernel<VANILLA><<<grid, kThreads, kRenderSmem, st>>>(*g, a);
-  NSR_CHECK_LAUNCH("nsr_neus_render_rays");
+  const int grid = (int)min((int64_t)nsr_sm_count() * kCtasPerSm<FD>, (a.n_rays + kNeusTcWarps - 1) / kNeusTcWarps);
+  neus_render_rays_kernel<VANILLA, FD><<<grid, kThreads, kRenderSmem<FD>, st>>>(*g, a);
+  NSR_CHECK_LAUNCH(name);
   return 0;
+}
+
+// both entry points: field_state is n_active (analytic field) or fd_state (finite-difference field)
+template <bool FD>
+int render_rays(const char* name, const nsr_grid_t* g, const float* rays, const uint32_t* masks, int32_t words, const float* t_min,
+                const int32_t* counts, const int32_t* bin_counts, const int32_t* order_bins, float step, const void* table_h, const float* W1,
+                const float* b1, const float* W2, const float* b2, float radius, int32_t n_out, const float* field_state,
+                const nsr_radiance_t* rp, int32_t vanilla, const void* rgb_params_h, const float* rgb_bias, const float* inv_s,
+                const float* cos_anneal, float* opacity, float* depth, float* comp_rgb, float* comp_normal, uint32_t* ticket, int64_t n_rays,
+                void* stream) {
+  NSR_REQUIRE(g != nullptr && g->n_levels == 16 && g->n_features == 2, "%s: needs a 16-level F=2 hash grid", name);
+  NSR_REQUIRE(n_out >= 1 && n_out <= 16, "%s: n_out must be in [1,16]", name);
+  NSR_REQUIRE(rp != nullptr && n_out == kFeat && rp->n_feat == kFeat && rp->n_extra == 3,
+              "%s: the colour input must be [feature (13) | SH4 (16) | normal (3)]", name);
+  NSR_REQUIRE(rp->act_mode >= 0 && rp->act_mode <= 2, "%s: act_mode must be 0, 1 or 2", name);
+  NSR_REQUIRE(words >= 1 && words <= kMaxWords, "%s: words must be in [1, %d]", name, kMaxWords);
+  NSR_REQUIRE(step > 0.f, "%s: step must be > 0", name);
+  NSR_REQUIRE(rays && masks && t_min && counts && bin_counts && order_bins && table_h && W1 && b1 && W2 && b2 && rgb_params_h && inv_s &&
+                  cos_anneal && opacity && depth && comp_rgb && comp_normal && ticket,
+              "%s: NULL argument", name);
+  NSR_REQUIRE(field_state != nullptr, FD ? "%s: fd_state (device {eps, eps^2, n_active}) is NULL" : "%s: NULL argument", name);
+  NSR_REQUIRE(!vanilla || rgb_bias != nullptr, "%s: the VanillaMLP colour network needs its bias", name);
+  if (n_rays == 0) return 0;
+  RenderArgs a;
+  a.rays = rays, a.masks = masks, a.t_min = t_min, a.counts = counts, a.bin_counts = bin_counts, a.order_bins = order_bins;
+  a.table = (const __half2*)table_h, a.W1 = W1, a.b1 = b1, a.W2 = W2, a.b2 = b2;
+  a.n_active = FD ? nullptr : field_state, a.fd_state = FD ? field_state : nullptr;
+  a.rgb_params = (const __half*)rgb_params_h, a.rgb_bias = rgb_bias, a.inv_s = inv_s, a.cos_anneal = cos_anneal;
+  a.opacity = opacity, a.depth = depth, a.comp_rgb = comp_rgb, a.comp_normal = comp_normal, a.ticket = ticket;
+  a.step = step, a.radius = radius, a.words = words, a.n_out = n_out, a.act_mode = rp->act_mode, a.n_rays = n_rays;
+  const cudaStream_t st = (cudaStream_t)stream;
+  return vanilla ? launch<true, FD>(g, a, st, name) : launch<false, FD>(g, a, st, name);
 }
 
 }  // namespace
@@ -228,24 +314,19 @@ extern "C" int nsr_neus_render_rays(const nsr_grid_t* g, const float* rays, cons
                                     const float* n_active, const nsr_radiance_t* rp, int32_t vanilla, const void* rgb_params_h,
                                     const float* rgb_bias, const float* inv_s, const float* cos_anneal, float* opacity, float* depth,
                                     float* comp_rgb, float* comp_normal, uint32_t* ticket, int64_t n_rays, void* stream) {
-  NSR_REQUIRE(g != nullptr && g->n_levels == 16 && g->n_features == 2, "nsr_neus_render_rays: needs a 16-level F=2 hash grid");
-  NSR_REQUIRE(n_out >= 1 && n_out <= 16, "nsr_neus_render_rays: n_out must be in [1,16]");
-  NSR_REQUIRE(rp != nullptr && n_out == kFeat && rp->n_feat == kFeat && rp->n_extra == 3,
-              "nsr_neus_render_rays: the colour input must be [feature (13) | SH4 (16) | normal (3)]");
-  NSR_REQUIRE(rp->act_mode >= 0 && rp->act_mode <= 2, "nsr_neus_render_rays: act_mode must be 0, 1 or 2");
-  NSR_REQUIRE(words >= 1 && words <= kMaxWords, "nsr_neus_render_rays: words must be in [1, %d]", kMaxWords);
-  NSR_REQUIRE(step > 0.f, "nsr_neus_render_rays: step must be > 0");
-  NSR_REQUIRE(rays && masks && t_min && counts && bin_counts && order_bins && table_h && W1 && b1 && W2 && b2 && rgb_params_h && n_active && inv_s &&
-                  cos_anneal && opacity && depth && comp_rgb && comp_normal && ticket,
-              "nsr_neus_render_rays: NULL argument");
-  NSR_REQUIRE(!vanilla || rgb_bias != nullptr, "nsr_neus_render_rays: the VanillaMLP colour network needs its bias");
-  if (n_rays == 0) return 0;
-  RenderArgs a;
-  a.rays = rays, a.masks = masks, a.t_min = t_min, a.counts = counts, a.bin_counts = bin_counts, a.order_bins = order_bins;
-  a.table = (const __half2*)table_h, a.W1 = W1, a.b1 = b1, a.W2 = W2, a.b2 = b2, a.n_active = n_active;
-  a.rgb_params = (const __half*)rgb_params_h, a.rgb_bias = rgb_bias, a.inv_s = inv_s, a.cos_anneal = cos_anneal;
-  a.opacity = opacity, a.depth = depth, a.comp_rgb = comp_rgb, a.comp_normal = comp_normal, a.ticket = ticket;
-  a.step = step, a.radius = radius, a.words = words, a.n_out = n_out, a.act_mode = rp->act_mode, a.n_rays = n_rays;
-  const cudaStream_t st = (cudaStream_t)stream;
-  return vanilla ? launch<true>(g, a, st) : launch<false>(g, a, st);
+  return render_rays<false>("nsr_neus_render_rays", g, rays, masks, words, t_min, counts, bin_counts, order_bins, step, table_h, W1, b1, W2, b2,
+                            radius, n_out, n_active, rp, vanilla, rgb_params_h, rgb_bias, inv_s, cos_anneal, opacity, depth, comp_rgb,
+                            comp_normal, ticket, n_rays, stream);
+}
+
+extern "C" int nsr_neus_render_rays_fd(const nsr_grid_t* g, const float* rays, const uint32_t* masks, int32_t words, const float* t_min,
+                                       const int32_t* counts, const int32_t* bin_counts, const int32_t* order_bins, float step,
+                                       const void* table_h, const float* W1, const float* b1, const float* W2, const float* b2, float radius,
+                                       int32_t n_out, const float* fd_state, const nsr_radiance_t* rp, int32_t vanilla,
+                                       const void* rgb_params_h, const float* rgb_bias, const float* inv_s, const float* cos_anneal,
+                                       float* opacity, float* depth, float* comp_rgb, float* comp_normal, uint32_t* ticket, int64_t n_rays,
+                                       void* stream) {
+  return render_rays<true>("nsr_neus_render_rays_fd", g, rays, masks, words, t_min, counts, bin_counts, order_bins, step, table_h, W1, b1, W2,
+                           b2, radius, n_out, fd_state, rp, vanilla, rgb_params_h, rgb_bias, inv_s, cos_anneal, opacity, depth, comp_rgb,
+                           comp_normal, ticket, n_rays, stream);
 }

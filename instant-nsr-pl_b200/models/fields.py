@@ -146,12 +146,18 @@ class VolumeSDF(BaseImplicitGeometry):
 
     def fused_render_unsupported(self):
         """None when NeuS eval rendering can run this field inside the per-ray kernel (ops.neus_render_rays: the fused analytic
-        field with a 13-wide output), else why it keeps the per-sample path (a message)."""
+        field, or with the opt-in key ``fused_render_fd: true`` the fused finite-difference field, with a 13-wide output), else why it
+        keeps the per-sample path (a message)."""
         if self.grad_type != 'analytic':
-            return 'finite-difference normals (neuralangelo) evaluate a seven-point stencil per sample: per-sample eval path'
-        if self._progressive and not self.config.get('fused_progressive', False):
+            if self.grad_type != 'finite_difference' or not self.config.get('fused_render_fd', False):
+                return ('finite-difference normals (neuralangelo) evaluate a seven-point stencil per sample: per-sample eval path unless '
+                        'the geometry sets fused_render_fd: true')
+            if not self._fused_fd:
+                return ('the geometry is not the fused finite-difference SDF field shape (include_xyz HashGrid or ProgressiveBandHashGrid '
+                        'L=16 F=2 + sphere-init VanillaMLP 35 -> 64 -> n_out, fused: true)')
+        elif self._progressive and not self.config.get('fused_progressive', False):
             return 'a ProgressiveBandHashGrid runs the fused field only with fused_progressive: true'
-        if not self._fused:
+        elif not self._fused:
             return ('the geometry is not the fused SDF field shape (include_xyz HashGrid L=16 F=2 + sphere-init VanillaMLP 35 -> 64 -> n_out, '
                     'analytic normals)')
         if self.n_output_dims != 13:
@@ -189,11 +195,16 @@ class VolumeSDF(BaseImplicitGeometry):
         rv = [v if self.training else v.detach() for v in rv]
         return rv[0] if len(rv) == 1 else rv
 
+    def _require_fd_eps(self):
+        """the stencil's step lives in _fd_state from the first update_step on"""
+        if self._finite_difference_eps is None:
+            raise RuntimeError('VolumeSDF: finite-difference step not set -- call update_step() before the first forward')
+
     def _forward_fused_fd(self, points, with_grad, with_feature, with_laplace):
         from .. import ops
         stencil = with_grad or with_laplace
-        if stencil and self._finite_difference_eps is None:
-            raise RuntimeError('VolumeSDF: finite-difference step not set -- call update_step() before the first forward')
+        if stencil:
+            self._require_fd_eps()
         enc = self._fd_grid()
         shape = points.shape[:-1]
         W1, b1, W2, b2 = self._effective_weights()

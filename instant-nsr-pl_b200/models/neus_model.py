@@ -349,7 +349,8 @@ class NeuSModel(BaseModel):
 
     def fused_render_unsupported(self):
         """None when eval-mode forward() renders through the per-ray kernel (ops.neus_render_rays; model config key
-        ``fused_render: true``), else why it keeps the per-sample path of chunk_batch(forward_) (a message)."""
+        ``fused_render: true``, plus the geometry key ``fused_render_fd: true`` for finite-difference normals), else why it keeps the
+        per-sample path of chunk_batch(forward_) (a message)."""
         cfg = self.config
         if not cfg.get('fused_render', False):
             return 'fused_render is off'
@@ -390,7 +391,12 @@ class NeuSModel(BaseModel):
             self._cos_dev = torch.full((1,), float(self.cos_anneal_ratio), device=dev)
         enc = geo._fd_grid()
         W1, b1, W2, b2 = geo._effective_weights()
-        n_active = geo._fd_state[2:] if geo._progressive else torch.full((1,), 16.0, device=dev)
+        fd_state = None
+        if geo.grad_type == 'finite_difference':   # eps and n_active from the device state update_step refreshes
+            geo._require_fd_eps()
+            fd_state, n_active = geo._fd_state, None
+        else:
+            n_active = geo._fd_state[2:] if geo._progressive else torch.full((1,), 16.0, device=dev)
         inv_s = self.variance.inv_s.clip(1e-6, 1e6).reshape(1)
         if spec.vanilla:
             weights, rgb_bias = ops.pack_vanilla_radiance(tex.network.linear_params())
@@ -403,7 +409,7 @@ class NeuSModel(BaseModel):
         for s in range(0, rays.shape[0], chunk):
             r = rays[s:s + chunk]
             fg.append(ops.neus_render_rays(ms, r, grid.bits(), grid.coarse_bits(), cap_per_ray, enc.grid, geo.radius, enc._params_half(), W1, b1,
-                                           W2, b2, n_active, spec, rgb_params, rgb_bias, inv_s, self._cos_dev))
+                                           W2, b2, n_active, spec, rgb_params, rgb_bias, inv_s, self._cos_dev, fd_state=fd_state))
             if bg_fused is not None:
                 o = bg_fused.render(r, None, static=True)
                 off = bg_fused.last_offsets_k

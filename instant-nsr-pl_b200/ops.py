@@ -872,16 +872,19 @@ def march_masks_static(ms, rays, jitter, bits, coarse_bits, cap_per_ray, cap):
 
 
 def neus_render_rays(ms, rays, bits, coarse_bits, cap_per_ray, grid_spec, radius, table_h, W1, b1, W2, b2, n_active, rspec, rgb_params_h,
-                     rgb_bias, inv_s, cos_anneal):
+                     rgb_bias, inv_s, cos_anneal, fd_state=None):
     """NeuS eval render of a pass of rays (NeuSModel.forward_ in eval mode, models/neus.py:205-243): lattice marcher (nsr_march_rays_alloc,
     AABB, cone 0; ms = march_struct) -> one kernel per ray warp (nsr_neus_render_rays).  No host sync; scratch is per ray only (masks
     4 * ceil(cap_per_ray / 32) B, t_min, counts, slice offsets and the longest-first queue).  W1 [64,35], b1, W2 [13,64], b2: the SDF
     network (effective weights); n_active: float32 CUDA tensor of one entry (active hash levels, 16 for a plain HashGrid); rspec: a
     RadianceSpec(13, 3, mode[, vanilla]); rgb_params_h fp16 [7168] and rgb_bias (VanillaMLP: f32 [144], else None); inv_s (clipped) and
     cos_anneal: float32 CUDA tensors of one entry.  -> dict(opacity [N,1], depth [N,1], comp_rgb [N,3] (before the background),
-    comp_normal [N,3] (un-normalised), counts int32 [N] = marched samples per ray)."""
+    comp_normal [N,3] (un-normalised), counts int32 [N] = marched samples per ray).
+    fd_state (float32 CUDA tensor {eps, eps^2, n_active}, VolumeSDF._fd_state): the finite-difference field (nsr_neus_render_rays_fd,
+    the Neuralangelo geometry) instead of the analytic one; n_active is then ignored (pass None)."""
     import ctypes
-    check_cuda(rays, bits, table_h, W1, W2, n_active, rgb_params_h, inv_s, cos_anneal, what='neus_render_rays')
+    field_state = n_active if fd_state is None else fd_state
+    check_cuda(rays, bits, table_h, W1, W2, field_state, rgb_params_h, inv_s, cos_anneal, what='neus_render_rays')
     rays = contig(rays.detach(), torch.float32)
     n, dev = rays.shape[0], rays.device
     words = (int(cap_per_ray) + 31) // 32
@@ -898,9 +901,10 @@ def neus_render_rays(ms, rays, bits, coarse_bits, cap_per_ray, grid_spec, radius
         lib.call('nsr_march_rays_alloc', ctypes.byref(ms), ptr(rays), None, ptr(bits), ptr(coarse_bits), ptr(masks), words, ptr(t_min),
                  ptr(counts), ptr(offsets), ptr(alloc_total), ptr(bin_counts), ptr(order_bins), n, stream())
         f32 = lambda t: contig(t.detach(), torch.float32)
-        lib.call('nsr_neus_render_rays', grid_spec.ref(), ptr(rays), ptr(masks), words, ptr(t_min), ptr(counts), ptr(bin_counts), ptr(order_bins),
-                 float(ms.step), ptr(table_h), ptr(f32(W1)), ptr(f32(b1)), ptr(f32(W2)), ptr(f32(b2)), float(radius), int(W2.shape[0]),
-                 ptr(n_active), rspec.ref(), int(rspec.vanilla), ptr(rgb_params_h), ptr(None if rgb_bias is None else f32(rgb_bias)),
+        lib.call('nsr_neus_render_rays' if fd_state is None else 'nsr_neus_render_rays_fd', grid_spec.ref(), ptr(rays), ptr(masks), words,
+                 ptr(t_min), ptr(counts), ptr(bin_counts), ptr(order_bins), float(ms.step), ptr(table_h), ptr(f32(W1)), ptr(f32(b1)),
+                 ptr(f32(W2)), ptr(f32(b2)), float(radius), int(W2.shape[0]), ptr(field_state), rspec.ref(), int(rspec.vanilla),
+                 ptr(rgb_params_h), ptr(None if rgb_bias is None else f32(rgb_bias)),
                  ptr(f32(inv_s.reshape(1))), ptr(f32(cos_anneal.reshape(1))), ptr(opacity), ptr(depth), ptr(comp_rgb), ptr(comp_normal),
                  ptr(ticket), n, stream())
     return {'opacity': opacity, 'depth': depth, 'comp_rgb': comp_rgb, 'comp_normal': comp_normal, 'counts': counts}
