@@ -322,6 +322,19 @@ int nsr_nerf_rays_fwd(const nsr_nerf_t* f, const float* rays, const uint32_t* ma
                       void* enc_save_h, float* sigmas, float* rgbs, float* weights, float* trans, int32_t* kidx, float* acc_rgb,
                       float* opacity, float* depth, int32_t* kept, uint32_t* ticket, int64_t n_rays, const int32_t* counts,
                       const int32_t* bin_counts, int32_t* kept_blocks, void* stream);
+/* nsr_nerf_render_rays: NeRFModel.forward_ in eval mode (models/nerf.py:82-109, randomized = False) for a pass of rays, on the kernel of
+ * nsr_nerf_rays_fwd without its per-sample outputs: writes per ray only acc_rgb [n,3] (before the background), opacity [n], depth [n]
+ * and kept [n] (samples with T >= early_stop_eps).  Groups of 32 consecutive marched samples and early ray termination as nsr_visibility
+ * scans them, so the kept set is the two-pass path's.  f->contraction must equal m->contraction and selects the samples:
+ *   0 (AABB, m->cone_angle == 0): masks / t_start (= t_min) / counts / bin_counts / order_bins as nsr_march_rays_alloc wrote them (rays
+ *     taken longest-first), t = fma(k, m->step, t_start), words in [1, 64];
+ *   2 (UN_BOUNDED_SPHERE): masks / t_start / counts of nsr_march_cone_mask, bin_counts / order_bins NULL (rays taken in ticket order);
+ *     sample k is step k of the marcher's chain from t_start with m->step and m->cone_angle, bit for bit; words in [1, 96].
+ * ticket: device uint32, zero on entry.  n_rays == 0 is a no-op. */
+int nsr_nerf_render_rays(const nsr_nerf_t* f, const nsr_march_t* m, const float* rays, const uint32_t* masks, int32_t words,
+                         const float* t_start, const int32_t* counts, const int32_t* bin_counts, const int32_t* order_bins,
+                         float early_stop_eps, const void* dparams_h, const void* cparams_h, float* acc_rgb, float* opacity,
+                         float* depth, int32_t* kept, uint32_t* ticket, int64_t n_rays, void* stream);
 /* loose -> packed copy of the kept samples (exact-size ray_indices / t_starts / t_ends / weights of the reference's dict). */
 int nsr_pack_kept(const int64_t* offsets_m, const int64_t* offsets_k, const float* t_min, float step, const int32_t* kidx,
                   const float* weights, int32_t* ray_indices_k, float* t_starts_k, float* t_ends_k, float* weights_k /* may be NULL */,

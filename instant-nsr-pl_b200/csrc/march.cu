@@ -292,25 +292,9 @@ __global__ void __launch_bounds__(kMarchWarps * 32) march_rays_expand_kernel(nsr
 // ------------------------------------------------------------------------------------------------
 // Fused-path marcher for cone_angle > 0 (unbounded scenes): march_seq_kernel's serial recurrence, one warp per ray.  The step
 // t1 = t0 + min(max(t0 * cone, step), 1e10) depends on the previous one, so it is not reassociated: every lane runs the SAME fp32
-// chain over a 32-step chunk (arithmetic only, no loads) and lane k keeps step k; the 32 occupancy tests of a chunk -- the loads --
-// then run in parallel.  The expand pass recomputes the chain instead of storing t per chunk.
+// chain over a 32-step chunk (arithmetic only, no loads) and lane k keeps step k (nsr_cone_chunk, march.cuh); the 32 occupancy tests of
+// a chunk -- the loads -- then run in parallel.  The expand pass recomputes the chain instead of storing t per chunk.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float cone_next(float t0, float cone, float step) { return t0 + fminf(fmaxf(t0 * cone, step), 1e10f); }
-
-// advance the chain by 32 steps from t (chunk start); lane `lane` receives its step [t0, t1)
-__device__ __forceinline__ float cone_chunk(float t, float cone, float step, int lane, float& t0, float& t1) {
-#pragma unroll
-  for (int k = 0; k < 32; ++k) {
-    const float tn = cone_next(t, cone, step);
-    if (k == lane) {
-      t0 = t;
-      t1 = tn;
-    }
-    t = tn;
-  }
-  return t;
-}
-
 __global__ void __launch_bounds__(kMarchWarps * 32) march_cone_mask_kernel(nsr_march_t p, const float* __restrict__ rays,
                                                                            const float* __restrict__ jitter, const float* __restrict__ t_min_in,
                                                                            const float* __restrict__ t_max_in, float near, float far,
@@ -332,7 +316,7 @@ __global__ void __launch_bounds__(kMarchWarps * 32) march_cone_mask_kernel(nsr_m
   int cnt = 0;
   for (int w = 0; w < words; ++w) {
     float t0 = 0.f, t1 = 0.f;
-    t = cone_chunk(t, cone, step, lane, t0, t1);
+    t = nsr_cone_chunk(t, cone, step, lane, t0, t1);
     const float tm = (t0 + t1) * 0.5f;
     const bool valid = tm < tmax;
     const bool occ = valid && occupied(p, bits, __fmaf_rn(tm, dx, ox), __fmaf_rn(tm, dy, oy), __fmaf_rn(tm, dz, oz));
@@ -364,7 +348,7 @@ __global__ void __launch_bounds__(kMarchWarps * 32) march_cone_expand_kernel(nsr
   int64_t base = beg;
   for (int w = 0; w < words && base < end && base < cap; ++w) {
     float t0 = 0.f, t1 = 0.f;
-    t = cone_chunk(t, cone, step, lane, t0, t1);
+    t = nsr_cone_chunk(t, cone, step, lane, t0, t1);
     const uint32_t m = mrow[w];
     if ((m >> lane) & 1u) {
       const int64_t pos = base + __popc(m & ((1u << lane) - 1u));

@@ -11,6 +11,12 @@
 // expand kernels.  Per-ray outputs are plain stores (no atomics: bit-reproducible); kept samples of ray r land at
 // offsets_m[r] + j (j < kept[r]) in the per-sample buffers ("loose" layout: a kept prefix per ray).
 // The kept set is identical to the two-pass path: same density code, same 32-sample chunking of the scan.
+//
+// Two template parameters give the eval renderer (nsr_nerf_render_rays) from the same body:
+//   CONE:  samples are the cone marcher's steps under UN_BOUNDED_SPHERE (masks of nsr_march_cone_mask: bit k of a ray = step k of the
+//          chain t1 = t0 + min(max(t0 * cone, step), 1e10) from t_start) instead of the AABB lattice t = fma(k, step, t_min);
+//   STORE: per-sample outputs (training) or per-ray outputs only (eval: acc_rgb, opacity, depth, kept).
+#include "march.cuh"
 #include "nerf_fused.cuh"
 
 namespace {
@@ -18,6 +24,7 @@ namespace {
 constexpr int kWarps = 8;
 constexpr int kThreads = kWarps * 32;
 constexpr int kMaxWords = 64;  // mask words per ray held in two registers per lane (<= 2048 lattice points)
+constexpr int kMaxWordsCone = 96;  // cone form: three registers per lane (nerf-colmap's step bound is 2073 = 65 words)
 // per-warp scratch (halves): A tile [32][40] + SH tile [32][24] + sigma (32 f32) + rgb (32 x 4 f32)
 constexpr int kWarpHalves = 32 * NF_LD32 + 32 * 24 + 64 + 256;
 constexpr size_t kSmemBytes = (size_t)(NF_W_TOTAL + kWarps * kWarpHalves) * sizeof(__half);
@@ -47,6 +54,7 @@ struct RaysFwdArgs {
   float step, early_stop_eps;
   int words;
   int64_t n_rays;
+  float cone;                  // CONE: cone angle of the marcher
 };
 
 __device__ __forceinline__ float warp_incl_prod(float v, int lane) {
@@ -68,6 +76,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 constexpr int kMinBlocks = 2;
 // levels whose 8 corner loads are issued together (8 levels measured no faster and spilled 120 B)
 constexpr int kGatherBatch = 4;
+template <bool CONE, bool STORE>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) nerf_rays_fwd_kernel(const __grid_constant__ nsr_nerf_t P, const RaysFwdArgs a) {
   extern __shared__ __align__(16) __half smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, c = lane & 3;
@@ -98,11 +107,12 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) nerf_rays_fwd_kernel(con
     } else if (a.order != nullptr) {
       ray = __ldg(a.order + ray);
     }
-    // ---- the ray's occupancy mask: lane w holds words w and w+32
+    // ---- the ray's occupancy mask: lane w holds words w and w+32 (cone form: and w+64)
     const uint32_t mw0 = lane < a.words ? __ldg(a.masks + ray * a.words + lane) : 0u;
     const uint32_t mw1 = lane + 32 < a.words ? __ldg(a.masks + ray * a.words + lane + 32) : 0u;
-    const int64_t base = a.offsets_m[ray];
-    const int total = a.counts != nullptr ? __ldg(a.counts + ray) : (int)(a.offsets_m[ray + 1] - base);
+    const uint32_t mw2 = CONE && lane + 64 < a.words ? __ldg(a.masks + ray * a.words + lane + 64) : 0u;
+    const int64_t base = STORE ? a.offsets_m[ray] : 0;
+    const int total = (!STORE || a.counts != nullptr) ? __ldg(a.counts + ray) : (int)(a.offsets_m[ray + 1] - base);
     float o_acc = 0.f, d_acc = 0.f, r_acc = 0.f, g_acc = 0.f, b_acc = 0.f;
     int kept = 0;
     if (total > 0) {
@@ -125,18 +135,33 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) nerf_rays_fwd_kernel(con
       sp[1] = sh1;
       int cur_w = 0;
       uint32_t cur_m = __shfl_sync(0xffffffffu, mw0, 0);
+      // cone form: the chain's steps of the cursor's word (lane j holds step j) and the next word's first t.  The cursor carries the chain
+      // across words; every word it passes, occupied or not, costs the 32-step chain (as in nsr_march_cone_expand).
+      float cw0 = 0.f, cw1 = 0.f, chain_t = tmin;
+      if (CONE) chain_t = nsr_cone_chunk(chain_t, a.cone, a.step, lane, cw0, cw1);
       for (int b0 = 0; b0 < total; b0 += 32) {
         const int s_idx = b0 + lane;
-        // next 32 set bits of the mask (warp-uniform cursor over the words; lane j takes the j-th of them)
+        // next 32 set bits of the mask (warp-uniform cursor over the words; lane j takes the j-th of them).  The cone form stops at the
+        // ray's count: nsr_march_cone_mask leaves the words behind its last step unwritten.
+        const int need = CONE ? min(32, total - b0) : 32;
         int k = -1, filled = 0;
-        while (filled < 32) {
+        float ct0 = 0.f, ct1 = 0.f;
+        while (filled < need) {
           if (cur_m == 0u) {
             if (++cur_w >= a.words) break;
-            cur_m = cur_w < 32 ? __shfl_sync(0xffffffffu, mw0, cur_w) : __shfl_sync(0xffffffffu, mw1, cur_w - 32);
+            cur_m = cur_w < 32 ? __shfl_sync(0xffffffffu, mw0, cur_w)
+                    : (!CONE || cur_w < 64) ? __shfl_sync(0xffffffffu, mw1, cur_w - 32) : __shfl_sync(0xffffffffu, mw2, cur_w - 64);
+            if (CONE) chain_t = nsr_cone_chunk(chain_t, a.cone, a.step, lane, cw0, cw1);
             continue;
           }
-          const int cnt = __popc(cur_m), take = min(cnt, 32 - filled);
+          const int cnt = __popc(cur_m), take = min(cnt, need - filled);
           if (lane >= filled && lane < filled + take) k = cur_w * 32 + (int)__fns(cur_m, 0, lane - filled + 1);
+          if (CONE) {  // the lane taking step `bit` of this word gets [t0, t1) from lane `bit`
+            const bool mine = lane >= filled && lane < filled + take;
+            const int bit = mine ? k - cur_w * 32 : 0;
+            const float u0 = __shfl_sync(0xffffffffu, cw0, bit), u1 = __shfl_sync(0xffffffffu, cw1, bit);
+            if (mine) ct0 = u0, ct1 = u1;
+          }
           if (take == cnt) {
             cur_m = 0u;
           } else {
@@ -147,11 +172,16 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) nerf_rays_fwd_kernel(con
         }
         const bool valid = k >= 0;
         if (!valid) k = 0;
-        // identical expression to nsr_march_rays_expand / march_lattice_kernel: t0 = fma(k, step, t_min)
-        const float t0 = __fmaf_rn((float)k, a.step, tmin), t1 = __fmaf_rn((float)k + 1.f, a.step, tmin);
+        // identical expression to nsr_march_rays_expand / march_lattice_kernel: t0 = fma(k, step, t_min); cone form: the marcher's chain
+        const float t0 = CONE ? ct0 : __fmaf_rn((float)k, a.step, tmin), t1 = CONE ? ct1 : __fmaf_rn((float)k + 1.f, a.step, tmin);
         const float mid = (t0 + t1) * 0.5f;
         uint32_t f[16];
-        if (valid) {
+        if (valid && CONE) {
+          // position and contraction of the two-pass contracted kernels (nf_sample_position<NF_UNBOUNDED_SPHERE>)
+          float x = fmaf(dx, mid, ox), y = fmaf(dy, mid, oy), z = fmaf(dz, mid, oz);
+          nf_contract<NF_UNBOUNDED_SPHERE>(P, x, y, z);
+          nf_gather_batched<16, kGatherBatch>(P.grid, table, x, y, z, f);
+        } else if (valid) {
           const float x = (fmaf(dx, mid, ox) + P.radius) * inv, y = (fmaf(dy, mid, oy) + P.radius) * inv,
                       z = (fmaf(dz, mid, oz) + P.radius) * inv;
           nf_gather_batched<16, kGatherBatch>(P.grid, table, x, y, z, f);   // 8 kGatherBatch loads per lane in flight
@@ -160,7 +190,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) nerf_rays_fwd_kernel(con
           for (int l = 0; l < 16; ++l) f[l] = 0u;
         }
         nf_store_row32(At, lane, f);
-        if (a.enc_save != nullptr && valid) {  // rows past the kept prefix are written too but never read
+        if (STORE && a.enc_save != nullptr && valid) {  // rows past the kept prefix are written too but never read
           uint4* e = reinterpret_cast<uint4*>(a.enc_save + (base + s_idx) * 32);
           e[0] = make_uint4(f[0], f[1], f[2], f[3]);
           e[1] = make_uint4(f[4], f[5], f[6], f[7]);
@@ -244,14 +274,16 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) nerf_rays_fwd_kernel(con
           r_acc += w * cr;
           g_acc += w * cg;
           b_acc += w * cb;
-          const int64_t p = base + s_idx;
-          a.sigmas[p] = sigma;
-          a.weights[p] = w;
-          a.trans[p] = T;
-          a.kidx_out[p] = k;
-          a.rgbs[p * 3 + 0] = cr;
-          a.rgbs[p * 3 + 1] = cg;
-          a.rgbs[p * 3 + 2] = cb;
+          if (STORE) {
+            const int64_t p = base + s_idx;
+            a.sigmas[p] = sigma;
+            a.weights[p] = w;
+            a.trans[p] = T;
+            a.kidx_out[p] = k;
+            a.rgbs[p * 3 + 0] = cr;
+            a.rgbs[p * 3 + 1] = cg;
+            a.rgbs[p * 3 + 2] = cb;
+          }
         }
         kept += __popc(__ballot_sync(0xffffffffu, keep));
         carry *= __shfl_sync(0xffffffffu, incl, 31);
@@ -271,7 +303,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) nerf_rays_fwd_kernel(con
       a.acc_rgb[ray * 3 + 1] = g_acc;
       a.acc_rgb[ray * 3 + 2] = b_acc;
       a.kept[ray] = kept;
-      if (a.kept_blocks != nullptr && kept > 0) atomicAdd(a.kept_blocks + (ray >> 8), kept);
+      if (STORE && a.kept_blocks != nullptr && kept > 0) atomicAdd(a.kept_blocks + (ray >> 8), kept);
     }
     __syncwarp();
   }
@@ -413,6 +445,26 @@ __global__ void __launch_bounds__(256) ray_bwd_loose_kernel(const int64_t* __res
   }
 }
 
+template <bool CONE, bool STORE>
+int reserve_smem(const char* name) {
+  static thread_local bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(nerf_rays_fwd_kernel<CONE, STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    if (e != cudaSuccess) {
+      nsr_set_error("%s: cannot reserve %zu B shared memory: %s", name, kSmemBytes, cudaGetErrorString(e));
+      return 2;
+    }
+    attr_set = true;
+  }
+  return 0;
+}
+
+// persistent grid: two CTAs per SM, fewer when there are fewer rays than warps
+int rays_grid(int64_t n_rays) {
+  const int64_t want = (n_rays + kWarps - 1) / kWarps;
+  return (int)min((int64_t)nsr_sm_count() * 2, want > 0 ? want : (int64_t)1);
+}
+
 }  // namespace
 
 extern "C" int nsr_nerf_rays_fwd(const nsr_nerf_t* f, const float* rays, const uint32_t* masks, int32_t words, const float* t_min,
@@ -427,25 +479,53 @@ extern "C" int nsr_nerf_rays_fwd(const nsr_nerf_t* f, const float* rays, const u
   NSR_REQUIRE(words >= 1 && words <= kMaxWords, "nsr_nerf_rays_fwd: words must be in [1,%d]", kMaxWords);
   NSR_REQUIRE(ticket != nullptr && kept != nullptr, "nsr_nerf_rays_fwd: ticket / kept are required");
   if (n_rays == 0) return 0;
-  static thread_local bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(nerf_rays_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e != cudaSuccess) {
-      nsr_set_error("nsr_nerf_rays_fwd: cannot reserve %zu B shared memory: %s", kSmemBytes, cudaGetErrorString(e));
-      return 2;
-    }
-    attr_set = true;
-  }
+  if (int e = reserve_smem<false, true>("nsr_nerf_rays_fwd")) return e;
   RaysFwdArgs a;
   a.rays = rays; a.masks = masks; a.t_min = t_min; a.offsets_m = offsets_m; a.order = order; a.bin_counts = bin_counts; a.counts = counts; a.kept_blocks = kept_blocks;
   a.dparams = (const __half*)dparams_h; a.cparams = (const __half*)cparams_h; a.enc_save = (__half*)enc_save_h;
   a.sigmas = sigmas; a.rgbs = rgbs; a.weights = weights; a.trans = trans; a.kidx_out = kidx;
   a.acc_rgb = acc_rgb; a.opacity = opacity; a.depth = depth; a.kept = kept; a.ticket = ticket;
-  a.step = step; a.early_stop_eps = early_stop_eps; a.words = words; a.n_rays = n_rays;
-  const int64_t want = (n_rays + kWarps - 1) / kWarps;
-  int grid = (int)min((int64_t)nsr_sm_count() * 2, want > 0 ? want : (int64_t)1);
-  nerf_rays_fwd_kernel<<<grid, kThreads, kSmemBytes, (cudaStream_t)stream>>>(*f, a);
+  a.step = step; a.early_stop_eps = early_stop_eps; a.words = words; a.n_rays = n_rays; a.cone = 0.f;
+  nerf_rays_fwd_kernel<false, true><<<rays_grid(n_rays), kThreads, kSmemBytes, (cudaStream_t)stream>>>(*f, a);
   NSR_CHECK_LAUNCH("nsr_nerf_rays_fwd");
+  return 0;
+}
+
+extern "C" int nsr_nerf_render_rays(const nsr_nerf_t* f, const nsr_march_t* m, const float* rays, const uint32_t* masks, int32_t words,
+                                    const float* t_start, const int32_t* counts, const int32_t* bin_counts, const int32_t* order_bins,
+                                    float early_stop_eps, const void* dparams_h, const void* cparams_h, float* acc_rgb, float* opacity,
+                                    float* depth, int32_t* kept, uint32_t* ticket, int64_t n_rays, void* stream) {
+  NSR_REQUIRE(f != nullptr && m != nullptr, "nsr_nerf_render_rays: field / march descriptor is NULL");
+  NSR_REQUIRE(f->grid.n_levels == 16 && f->grid.n_features == 2 && f->feature_dim == 16 && f->density_hidden == 1 && f->color_hidden == 2,
+              "nsr_nerf_render_rays: needs L=16, F=2, feature_dim=16, hidden layers 1/2");
+  NSR_REQUIRE(f->contraction == m->contraction, "nsr_nerf_render_rays: field contraction %d != march contraction %d", f->contraction,
+              m->contraction);
+  NSR_REQUIRE(f->contraction == NF_AABB || f->contraction == NF_UNBOUNDED_SPHERE,
+              "nsr_nerf_render_rays: contraction type %d not implemented (AABB=0, UN_BOUNDED_SPHERE=2)", f->contraction);
+  const bool cone = f->contraction == NF_UNBOUNDED_SPHERE;
+  NSR_REQUIRE(m->step > 0.f && (cone ? m->cone_angle >= 0.f : m->cone_angle == 0.f),
+              "nsr_nerf_render_rays: needs step > 0 and cone_angle == 0 (AABB) / >= 0 (UN_BOUNDED_SPHERE)");
+  const int max_words = cone ? kMaxWordsCone : kMaxWords;
+  NSR_REQUIRE(words >= 1 && words <= max_words, "nsr_nerf_render_rays: words must be in [1,%d], got %d", max_words, words);
+  NSR_REQUIRE(bin_counts == nullptr || order_bins != nullptr, "nsr_nerf_render_rays: bin_counts needs order_bins");
+  NSR_REQUIRE(rays != nullptr && masks != nullptr && t_start != nullptr && counts != nullptr && dparams_h != nullptr && cparams_h != nullptr,
+              "nsr_nerf_render_rays: NULL input");
+  NSR_REQUIRE(acc_rgb != nullptr && opacity != nullptr && depth != nullptr && kept != nullptr && ticket != nullptr,
+              "nsr_nerf_render_rays: NULL output / ticket");
+  if (n_rays == 0) return 0;
+  RaysFwdArgs a = {};
+  a.rays = rays; a.masks = masks; a.t_min = t_start; a.counts = counts; a.bin_counts = bin_counts; a.order = order_bins;
+  a.dparams = (const __half*)dparams_h; a.cparams = (const __half*)cparams_h;
+  a.acc_rgb = acc_rgb; a.opacity = opacity; a.depth = depth; a.kept = kept; a.ticket = ticket;
+  a.step = m->step; a.early_stop_eps = early_stop_eps; a.words = words; a.n_rays = n_rays; a.cone = m->cone_angle;
+  if (cone) {
+    if (int e = reserve_smem<true, false>("nsr_nerf_render_rays")) return e;
+    nerf_rays_fwd_kernel<true, false><<<rays_grid(n_rays), kThreads, kSmemBytes, (cudaStream_t)stream>>>(*f, a);
+  } else {
+    if (int e = reserve_smem<false, false>("nsr_nerf_render_rays")) return e;
+    nerf_rays_fwd_kernel<false, false><<<rays_grid(n_rays), kThreads, kSmemBytes, (cudaStream_t)stream>>>(*f, a);
+  }
+  NSR_CHECK_LAUNCH("nsr_nerf_render_rays");
   return 0;
 }
 

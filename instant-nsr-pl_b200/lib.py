@@ -92,6 +92,7 @@ _SIGNATURES = {
     'nsr_march_cone_mask': [P, P, P, P, P, F32, F32, P, P, I32, P, P, I64, P],
     'nsr_march_cone_expand': [P, P, I32, P, P, P, P, P, I64, P, I64, P],
     'nsr_nerf_rays_fwd': [P, P, P, I32, P, P, P, F32, F32, P, P, P, P, P, P, P, P, P, P, P, P, P, I64, P, P, P, P],
+    'nsr_nerf_render_rays': [P, P, P, P, I32, P, P, P, P, F32, P, P, P, P, P, P, P, I64, P],
     'nsr_pack_kept': [P, P, P, F32, P, P, P, P, P, P, P, P, P, P, P, P, I32, I64, P],
     'nsr_pack_kept_scan': [P, P, P, P, F32, P, P, P, P, P, P, P, P, P, P, P, P, I32, I64, P, P],
     'nsr_nerf_ray_bwd_loose': [P, P, P, F32, P, P, P, P, P, P, P, P, P, P, P, P, P, I64, P],

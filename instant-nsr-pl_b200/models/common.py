@@ -1,6 +1,7 @@
 """Shared pieces of the drop-in models: BaseModel (models/base.py), activation table and trunc_exp
 (models/utils.py:53-97), scale_anything (:108-113), chunk_batch (:13-50), update_module_step
-(systems/utils.py:349-351), rank lookup (utils/misc.py:42-50)."""
+(systems/utils.py:349-351), rank lookup (utils/misc.py:42-50), and the per-slice
+num_samples layout of chunk_batch built from per-ray counts (slice_sums)."""
 import os
 from collections import defaultdict
 
@@ -132,6 +133,12 @@ def chunk_batch(func, chunk_size, move_to_cpu, *args, **kwargs):
     if kind in (tuple, list):
         return kind(merged[i] for i in range(width))
     return merged
+
+
+def slice_sums(per_ray, ray_chunk):
+    """chunk_batch's num_samples layout: one int32 entry per ``ray_chunk`` slice of the rays, the per-ray counts summed per slice."""
+    pad = (-per_ray.shape[0]) % ray_chunk
+    return F.pad(per_ray.to(torch.int64), (0, pad)).view(-1, ray_chunk).sum(1).to(torch.int32)
 
 
 def cleanup():

@@ -7,6 +7,9 @@ Two execution paths, identical results up to fp16 tolerance:
              (``nsr_b200.fused``), one launch per stage instead of ~40 torch/tcnn/nerfacc kernels.  The unbounded
              nerf-colmap shape (learned_background) takes it only with the config key ``fused_unbounded: true``.
   * composed: the per-op tcnn-/nerfacc-shaped modules in the order the reference calls them.
+
+Eval-mode forward() renders through the per-ray kernel (ops.nerf_render_rays) when the config sets ``fused_render: true`` and the fused
+path is selected; fused_render_unsupported() says why a config keeps chunk_batch(forward_).
 """
 import math
 
@@ -15,7 +18,8 @@ import torch
 from . import register, make
 from .. import nerfacc
 from ..nerfacc import ContractionType, OccupancyGrid, ray_marching, render_weight_from_density, accumulate_along_rays
-from .common import BaseModel, chunk_batch, update_module_step
+from .common import BaseModel, chunk_batch, slice_sums, update_module_step
+from .. import ops
 
 
 @register('nerf')
@@ -114,9 +118,44 @@ class NeRFModel(BaseModel):
             raise RuntimeError('static (sync-free) rendering needs the fused CUDA path')
         return self._render_composed(rays, jitter=jitter)
 
+    def fused_render_unsupported(self):
+        """None when eval-mode forward() renders through the per-ray kernel (ops.nerf_render_rays; model config key
+        ``fused_render: true``), else why it keeps the per-sample path of chunk_batch(forward_) (a message)."""
+        cfg = self.config
+        if not cfg.get('fused_render', False):
+            return 'fused_render is off'
+        if not cfg.grid_prune:
+            return 'the per-ray renderer marches the occupancy grid: needs grid_prune'
+        if self._fused is None:
+            if cfg.learned_background and not cfg.get('fused_unbounded', False):
+                return 'the unbounded scene renders on the fused kernels only with fused_unbounded: true'
+            return ('no fused executor: the field is not the fused shape (HashGrid L=16 F=2 + FullyFusedMLP networks, SH4 directions, '
+                    'trunc_exp density, sigmoid colour)')
+        return None
+
+    @torch.no_grad()
+    def _render_fused(self, rays):
+        """eval-mode forward() on the per-ray kernel: passes of config.render_chunk rays, outputs kept on the device and copied to the CPU
+        once; the dict of chunk_batch(forward_, ray_chunk, True, rays)."""
+        fz = self._fused
+        rays = rays.float().contiguous()
+        grid = self.occupancy_grid
+        bits, coarse = grid.bits(), grid.coarse_bits()
+        dh, ch = fz.dparams_half(), fz.cparams_half()
+        near, far = (max(0.0, fz.near), min(1e10, fz.far)) if fz.contracted else (0.0, 1e10)
+        chunk = int(self.config.get('render_chunk', 65536))
+        parts = [ops.nerf_render_rays(fz.struct, fz.march, rays[s:s + chunk], bits, coarse, fz.cap_per_ray, dh, ch, fz.early_stop_eps,
+                                      near, far) for s in range(0, rays.shape[0], chunk)]
+        acc_rgb, opacity, depth, kept = (torch.cat([p[k] for p in parts]) for k in ('acc_rgb', 'opacity', 'depth', 'kept'))
+        out = {'comp_rgb': acc_rgb + self.background_color * (1.0 - opacity), 'opacity': opacity, 'depth': depth, 'rays_valid': opacity > 0,
+               'num_samples': slice_sums(kept, self.config.ray_chunk)}
+        return {k: v.cpu() for k, v in out.items()}
+
     def forward(self, rays):
         if self.training:
             return {**self.forward_(rays)}
+        if rays.is_cuda and rays.shape[0] > 0 and self.fused_render_unsupported() is None:
+            return self._render_fused(rays)
         return {**chunk_batch(self.forward_, self.config.ray_chunk, True, rays)}
 
     def train(self, mode=True):

@@ -10,7 +10,7 @@ import torch.nn.functional as F
 from . import register, make
 from ..nerfacc import (ContractionType, OccupancyGrid, ray_marching, render_weight_from_density, render_weight_from_alpha,
                        accumulate_along_rays, ray_aabb_intersect)
-from .common import BaseModel, chunk_batch, update_module_step
+from .common import BaseModel, chunk_batch, slice_sums, update_module_step
 from .. import ops
 
 
@@ -71,12 +71,6 @@ def _long_keep_offsets(ray_indices):
 def _logistic_alpha(prev_sdf, next_sdf, inv_s):
     prev_cdf, next_cdf = torch.sigmoid(prev_sdf * inv_s), torch.sigmoid(next_sdf * inv_s)
     return ((prev_cdf - next_cdf + 1e-5) / (prev_cdf + 1e-5)).clip(0.0, 1.0)
-
-
-def slice_sums(per_ray, ray_chunk):
-    """chunk_batch's num_samples layout: one int32 entry per ``ray_chunk`` slice of the rays, the per-ray counts summed per slice."""
-    pad = (-per_ray.shape[0]) % ray_chunk
-    return F.pad(per_ray.to(torch.int64), (0, pad)).view(-1, ray_chunk).sum(1).to(torch.int32)
 
 
 def fused_eval_dict(fg, ray_chunk, background_color=None, bg=None):

@@ -908,3 +908,40 @@ def neus_render_rays(ms, rays, bits, coarse_bits, cap_per_ray, grid_spec, radius
                  ptr(f32(inv_s.reshape(1))), ptr(f32(cos_anneal.reshape(1))), ptr(opacity), ptr(depth), ptr(comp_rgb), ptr(comp_normal),
                  ptr(ticket), n, stream())
     return {'opacity': opacity, 'depth': depth, 'comp_rgb': comp_rgb, 'comp_normal': comp_normal, 'counts': counts}
+
+
+def nerf_render_rays(f, ms, rays, bits, coarse_bits, bound, dparams_h, cparams_h, early_stop_eps, near=0.0, far=1e10):
+    """NeRF eval render of a pass of rays (NeRFModel.forward_ in eval mode, models/nerf.py:82-109): marcher -> one kernel per ray warp
+    (nsr_nerf_render_rays).  f: the field's NerfT; ms: march_struct with the same contraction.  AABB (0): nsr_march_rays_alloc over bits /
+    coarse_bits, rays taken longest-first; UN_BOUNDED_SPHERE (2): nsr_march_cone_mask from ``near`` to ``far`` without jitter (coarse_bits
+    unused).  bound: marched samples per ray at most (words = ceil(bound / 32)).  No host sync; scratch is per ray only.
+    -> dict(acc_rgb [N,3] (before the background), opacity [N,1], depth [N,1], kept int32 [N] = samples with T >= early_stop_eps)."""
+    import ctypes
+    check_cuda(rays, bits, dparams_h, cparams_h, what='nerf_render_rays')
+    rays = contig(rays.detach(), torch.float32)
+    n, dev = rays.shape[0], rays.device
+    words = max(1, (int(bound) + 31) // 32)
+    cone = f.contraction == 2
+    zeros = torch.zeros(12, dtype=torch.int32, device=dev)   # one fill: alloc_total (uint64) | bin_counts [8] | ticket
+    alloc_total, bin_counts, ticket = zeros[0:2], zeros[2:10], zeros[10:11]
+    masks = torch.empty(n * words, dtype=torch.int32, device=dev)
+    t_start = torch.empty(n, device=dev)
+    counts = torch.empty(n, dtype=torch.int32, device=dev)
+    acc_rgb, opacity, depth = torch.empty(n, 3, device=dev), torch.empty(n, 1, device=dev), torch.empty(n, 1, device=dev)
+    kept = torch.empty(n, dtype=torch.int32, device=dev)
+    if n > 0:
+        mref = ctypes.byref(ms)
+        order_bins = None
+        if cone:
+            lib.call('nsr_march_cone_mask', mref, ptr(rays), None, None, None, float(near), float(far), ptr(bits), ptr(masks), words,
+                     ptr(t_start), ptr(counts), n, stream())
+            bin_counts = None
+        else:
+            offsets = torch.empty(n, dtype=torch.int64, device=dev)
+            order_bins = torch.empty(8 * n, dtype=torch.int32, device=dev)
+            lib.call('nsr_march_rays_alloc', mref, ptr(rays), None, ptr(bits), ptr(coarse_bits), ptr(masks), words, ptr(t_start), ptr(counts),
+                     ptr(offsets), ptr(alloc_total), ptr(bin_counts), ptr(order_bins), n, stream())
+        lib.call('nsr_nerf_render_rays', ctypes.byref(f), mref, ptr(rays), ptr(masks), words, ptr(t_start), ptr(counts), ptr(bin_counts),
+                 ptr(order_bins), float(early_stop_eps), ptr(dparams_h), ptr(cparams_h), ptr(acc_rgb), ptr(opacity), ptr(depth), ptr(kept),
+                 ptr(ticket), n, stream())
+    return {'acc_rgb': acc_rgb, 'opacity': opacity, 'depth': depth, 'kept': kept}
