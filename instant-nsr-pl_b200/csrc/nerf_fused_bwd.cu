@@ -7,8 +7,8 @@
 // levels) with 8-byte vector REDs into the fp32 gradient table, then split the five weight-gradient GEMMs
 // (dW = dPre^T * Act, K = 64 samples) over the 4 warps with register accumulators that persist for the whole
 // kernel; one atomicAdd per weight per CTA at the end (tcnn: split-K CUTLASS GEMMs over K = batch + reduction).
-// The split backward's network half (nerf_bwd_net_kernel, below) runs the same chain but hands the weight-gradient GEMMs to a wgmma
-// warpgroup.
+// The split backward's network half (nerf_bwd_net_kernel, below) runs the same chain as register-A wgmma on three chain warpgroups and
+// hands the weight-gradient GEMMs to a third warpgroup.
 #include "nerf_fused.cuh"
 #include "wgmma.cuh"
 
@@ -406,20 +406,26 @@ __global__ void __launch_bounds__(kThreads, kCtasPerSm) nerf_bwd_kernel(const __
 }
 
 // ==== network half of the split backward (nsr_nerf_field_bwd_net / _split) =====================================================
-// One CTA per SM, 12 warps, persistent over the CTA's 64-row tiles of packed rows (tile = blockIdx.x + it * gridDim.x):
-//   warps 0-3, 4-7   two chain groups that take the CTA's tiles in turn (group = it & 1).  A group runs the same warp-level code as
-//                    nerf_bwd_kernel -- mma.sync forward recompute and dgrad chain in registers, 16 rows per warp, the same fp16 rounding
-//                    points, ReLU masks and loss scale -- writes d(encoding) to global memory, and leaves every activation and
-//                    pre-activation gradient the weight gradients need in a tile slot, in wgmma's canonical no-swizzle layout.
-//                    Each group prefetches its next tile's inputs (cp.async, 7.5 KB) into its own stage while it computes.
-//   warps 8-11       one warpgroup that runs the five weight-gradient GEMMs of every tile (K = the tile's 64 rows) as wgmma.mma_async
+// One CTA per SM, 16 warps, persistent over the CTA's 64-row tiles of packed rows (tile = blockIdx.x + it * gridDim.x):
+//   warps 0-11       three chain warpgroups that take the CTA's tiles in turn (group = it % 3).  A group runs the chain of nerf_bwd_kernel
+//                    -- forward recompute and dgrad, activations in registers, 16 rows per warp, the same fp16 rounding points, ReLU
+//                    masks and loss scale -- but issues each layer as register-A wgmma.mma_async over the group's 64 rows: A is the
+//                    warps' m16n8k16 A fragments, B one canonical copy of the weights in shared memory (K-major for the forward, the
+//                    same copy MN-major for the dgrad), so the weights are read once per warpgroup and layer, not once per warp.
+//                    It writes d(encoding) to global memory and leaves every activation and pre-activation gradient the weight
+//                    gradients need in a tile slot, in wgmma's canonical no-swizzle layout.
+//                    Each group prefetches its next tile's inputs (cp.async, 7.5 KB) into its own stage while it computes.  Every layer
+//                    ends in a wait for its wgmma: three groups keep the tensor cores busy during one another's waits and epilogues.
+//   warps 12-15      one warpgroup that runs the five weight-gradient GEMMs of every tile (K = the tile's 64 rows) as wgmma.mma_async
 //                    with both operands read from the slot (MN-major descriptors over the K-major tiles: no transposes).  dDW2 and dCW3
 //                    (16 outputs) are computed transposed so that M = 64.  The 80 fp32 accumulators per thread live in registers for the
 //                    whole kernel; one atomicAdd per weight per CTA at the end.
-// Three slots form a ring (tile it -> slot it % 3): mbarrier FULL[s] hands a slot from its chain group to the warpgroup, EMPTY[s] back.
+// Three slots form a ring (tile it -> slot it % 3, so each group fills its own slot): mbarrier FULL[s] hands a slot from its chain group
+// to the warpgroup, EMPTY[s] back.  512 threads leave 128 registers per thread; neither role spills at that budget.
 // Rows past the live count hold zeros in every slot operand: their encodings and per-row inputs are zeroed in the stage, and every
 // layer maps zero inputs to zero.
-constexpr int kNetThreads = 384;
+constexpr int kChainGroups = 3;
+constexpr int kNetThreads = (kChainGroups + 1) * 128;
 // one tile slot (bytes), canonical [64][K] fp16 tiles
 constexpr int SL_X0 = 0;                    // [64][32] encoded features
 constexpr int SL_CI = SL_X0 + kRows * 32 * 2;   // [64][32] colour input: out16 | SH16
@@ -433,11 +439,17 @@ constexpr int SL_DG1 = SL_DG2 + kRows * 64 * 2; // [64][64]
 constexpr int SL_DH1 = SL_DG1 + kRows * 64 * 2; // [64][64]
 constexpr int kSlotBytes = SL_DH1 + kRows * 64 * 2;  // 61440
 constexpr int kNetSlots = 3;
-// CTA map (bytes): padded weights | slots | two input stages (encodings [64][40] halves + the per-row floats) | mbarriers
-constexpr int N_SLOTS = NF_W_TOTAL * 2;
+// CTA map (bytes): weights | slots | one input stage per chain group (encodings [64][40] halves + the per-row floats) | mbarriers
+// weights of both networks, canonical [out][in] fp16 tiles
+constexpr int NW_DW1 = 0;                      // [64][32]
+constexpr int NW_DW2 = NW_DW1 + 64 * 32 * 2;   // [16][64]
+constexpr int NW_CW1 = NW_DW2 + 16 * 64 * 2;   // [64][32]
+constexpr int NW_CW2 = NW_CW1 + 64 * 32 * 2;   // [64][64]
+constexpr int NW_CW3 = NW_CW2 + 64 * 64 * 2;   // [16][64]
+constexpr int N_SLOTS = NW_CW3 + 16 * 64 * 2;  // 20480
 constexpr int N_STAGE = N_SLOTS + kNetSlots * kSlotBytes;
 constexpr int kStageBytes = kRows * NF_LD32 * 2 + S_ROWF * 4;  // 7680
-constexpr int N_BARS = N_STAGE + 2 * kStageBytes;
+constexpr int N_BARS = N_STAGE + kChainGroups * kStageBytes;
 constexpr size_t kNetSmemBytes = N_BARS + 2 * kNetSlots * 8;
 static_assert(N_SLOTS % 128 == 0 && kSlotBytes % 128 == 0 && kStageBytes % 16 == 0 && N_BARS % 8 == 0, "alignment");
 static_assert(kNetSmemBytes <= 227 * 1024, "shared memory");
@@ -464,6 +476,38 @@ __device__ __forceinline__ void canon_store_afrag(const uint32_t (&a)[1][KT][4],
 }
 __device__ __forceinline__ void group_bar(int grp) { asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory"); }
 
+// row-major [rows][K] fp16 matrix (global) -> canonical smem tile
+__device__ __forceinline__ void canon_stage(uint8_t* dst, const __half* __restrict__ src, int rows, int K) {
+  const int vec_per_row = K / 8;
+  for (int i = threadIdx.x; i < rows * vec_per_row; i += blockDim.x) {
+    const int r = i / vec_per_row, kc = i % vec_per_row;
+    *reinterpret_cast<uint4*>(dst + nsr_canon_off(r, kc * 8, K)) = __ldg(reinterpret_cast<const uint4*>(src + (size_t)r * K) + kc);
+  }
+}
+
+// One chain layer over the warpgroup's 64 rows: acc = A . W^T (TB 0, forward: W [N out][K in] read K-major) or acc = A . W (TB 1,
+// dgrad: W [K out][ldw in] read MN-major, N <= ldw: the first N input columns).  A = this warp's 16 rows as KT m16n8k16 A fragments,
+// W = a canonical weight tile at shared address w with ldw halves per row; acc in the m16n8 C-fragment layout.  Returns with the
+// result in acc.
+template <int N, int KT, int TB>
+__device__ __forceinline__ void chain_gemm(float (&acc)[1][N / 8][4], const uint32_t (&a)[1][KT][4], uint32_t w, int ldw) {
+  float(&d)[N / 2] = *reinterpret_cast<float(*)[N / 2]>(&acc[0][0][0]);
+#pragma unroll
+  for (int kk = 0; kk < KT; ++kk)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) asm volatile("" ::"r"(a[0][kk][i]) : "memory");  // the A fragments are complete before the fence
+  nsr_wg_fence_regs(d);
+  nsr_wg_fence();
+#pragma unroll
+  for (int kk = 0; kk < KT; ++kk) {
+    const uint64_t db = TB ? nsr_wg_desc_mn(w, ldw, kk) : nsr_wg_desc(w + 256u * (uint32_t)kk, 128u, (uint32_t)(ldw / 8) * 128u);
+    nsr_wgmma_rs<N, TB>(d, a[0][kk], db, kk > 0 ? 1u : 0u);
+  }
+  nsr_wg_commit();
+  nsr_wg_wait0();
+  nsr_wg_fence_regs(d);
+}
+
 // flush one weight-gradient accumulator (m64nN layout) into dst[m * stride_m + n * stride_n]
 template <int R>
 __device__ __forceinline__ void net_flush(const float (&w)[R], float* dst, int stride_m, int stride_n, float inv_scale) {
@@ -484,7 +528,6 @@ __global__ void __launch_bounds__(kNetThreads, 1) nerf_bwd_net_kernel(const __ha
                                                                       uint32_t* __restrict__ denc_out) {
   const int64_t n = n_dev ? min(*n_dev, n_cap) : n_cap;
   extern __shared__ __align__(128) uint8_t smem_net[];
-  __half* W = reinterpret_cast<__half*>(smem_net);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (loss_scale <= 0.f) {  // automatic: the same rule as nerf_bwd_kernel
     const float amax = fmaxf(__ldg(amax_ptr), 1e-30f);
@@ -501,12 +544,17 @@ __global__ void __launch_bounds__(kNetThreads, 1) nerf_bwd_net_kernel(const __ha
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  nf_stage_weights(W, dparams, cparams, true);
+  canon_stage(smem_net + NW_DW1, dparams, 64, 32);
+  canon_stage(smem_net + NW_DW2, dparams + 64 * 32, 16, 64);
+  canon_stage(smem_net + NW_CW1, cparams, 64, 32);
+  canon_stage(smem_net + NW_CW2, cparams + 64 * 32, 64, 64);
+  canon_stage(smem_net + NW_CW3, cparams + 64 * 32 + 64 * 64, 16, 64);
+  nsr_proxy_fence();  // the chain's wgmmas read the weights through the async proxy
   __syncthreads();
   const int64_t n_tiles = (n + kRows - 1) / kRows;
   const int64_t my_tiles = n_tiles > (int64_t)blockIdx.x ? (n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
 
-  if (warp < 8) {
+  if (warp < 4 * kChainGroups) {
     // ================================ chain groups ================================
     const int grp = warp >> 2, gtid = threadIdx.x & 127, g = lane >> 2, c = lane & 3;
     const int r0 = (warp & 3) * 16;
@@ -521,7 +569,7 @@ __global__ void __launch_bounds__(kNetThreads, 1) nerf_bwd_net_kernel(const __ha
       cp_async_commit();
     };
     if (grp < my_tiles) fetch_tile(grp);
-    for (int64_t it = grp; it < my_tiles; it += 2) {
+    for (int64_t it = grp; it < my_tiles; it += kChainGroups) {
       const int s = (int)(it % kNetSlots);
       const int64_t row0 = ((int64_t)blockIdx.x + it * gridDim.x) * kRows;
       cp_async_wait_all();
@@ -562,17 +610,15 @@ __global__ void __launch_bounds__(kNetThreads, 1) nerf_bwd_net_kernel(const __ha
         dsr[hh] = rf[S_DS + r0 + g + hh * 8];
       }
       group_bar(grp);  // the whole group is done with the stage: refill it with the group's next tile
-      if (it + 2 < my_tiles) fetch_tile(it + 2);
+      if (it + kChainGroups < my_tiles) fetch_tile(it + kChainGroups);
 
       // ---- forward recompute
       uint32_t a_h1[1][4][4], a_o[1][1][4], a_g1[1][4][4], a_g2[1][4][4];
       float acc[1][8][4], acc16[1][2][4];
-      nsr_zero_acc(acc);
-      nsr_gemm_w<1, 2, 8>(acc, a_in, W + NF_OFF_DW1, NF_LD32);
+      chain_gemm<64, 2, 0>(acc, a_in, sbase + NW_DW1, 32);
       nsr_acc_to_afrag<1, 8>(acc, a_h1, NSR_ACT_RELU);
       canon_store_afrag<4>(a_h1, slot + SL_H1, 64, r0);
-      nsr_zero_acc(acc16);
-      nsr_gemm_w<1, 4, 2>(acc16, a_h1, W + NF_OFF_DW2, NSR_LD64);
+      chain_gemm<16, 4, 0>(acc16, a_h1, sbase + NW_DW2, 64);
       nsr_acc_to_afrag<1, 2>(acc16, a_o, NSR_ACT_NONE);
       canon_store_afrag<1>(a_o, slot + SL_CI, 32, r0);
       __syncwarp();
@@ -584,17 +630,14 @@ __global__ void __launch_bounds__(kNetThreads, 1) nerf_bwd_net_kernel(const __ha
           a_c[0][0][j] = a_o[0][0][j];
           a_c[0][1][j] = a_sh[0][0][j];
         }
-        nsr_zero_acc(acc);
-        nsr_gemm_w<1, 2, 8>(acc, a_c, W + NF_OFF_CW1, NF_LD32);
+        chain_gemm<64, 2, 0>(acc, a_c, sbase + NW_CW1, 32);
       }
       nsr_acc_to_afrag<1, 8>(acc, a_g1, NSR_ACT_RELU);
       canon_store_afrag<4>(a_g1, slot + SL_G1, 64, r0);
-      nsr_zero_acc(acc);
-      nsr_gemm_w<1, 4, 8>(acc, a_g1, W + NF_OFF_CW2, NSR_LD64);
+      chain_gemm<64, 4, 0>(acc, a_g1, sbase + NW_CW2, 64);
       nsr_acc_to_afrag<1, 8>(acc, a_g2, NSR_ACT_RELU);
       canon_store_afrag<4>(a_g2, slot + SL_G2, 64, r0);
-      nsr_zero_acc(acc16);
-      nsr_gemm_w<1, 4, 2>(acc16, a_g2, W + NF_OFF_CW3, NSR_LD64);
+      chain_gemm<16, 4, 0>(acc16, a_g2, sbase + NW_CW3, 64);
       // ---- d(rgb pre-activation) = d_rgb * s (1 - s), s = sigmoid(fp16(raw)); columns 0..2 only
       uint32_t a_dc3[1][1][4];
       {
@@ -622,16 +665,13 @@ __global__ void __launch_bounds__(kNetThreads, 1) nerf_bwd_net_kernel(const __ha
       }
       // ---- dgrad chain
       uint32_t a_d[1][4][4];
-      nsr_zero_acc(acc);
-      nsr_gemm_wt<1, 1, 8>(acc, a_dc3, W + NF_OFF_CW3, NSR_LD64);
+      chain_gemm<64, 1, 1>(acc, a_dc3, sbase + NW_CW3, 64);
       relu_mask_pack(acc, a_g2, a_d);
       canon_store_afrag<4>(a_d, slot + SL_DG2, 64, r0);
-      nsr_zero_acc(acc);
-      nsr_gemm_wt<1, 4, 8>(acc, a_d, W + NF_OFF_CW2, NSR_LD64);
+      chain_gemm<64, 4, 1>(acc, a_d, sbase + NW_CW2, 64);
       relu_mask_pack(acc, a_g1, a_d);
       canon_store_afrag<4>(a_d, slot + SL_DG1, 64, r0);
-      nsr_zero_acc(acc16);
-      nsr_gemm_wt<1, 4, 2>(acc16, a_d, W + NF_OFF_CW1, NF_LD32);  // first 16 input columns = the geometry features
+      chain_gemm<16, 4, 1>(acc16, a_d, sbase + NW_CW1, 32);  // first 16 input columns = the geometry features
       if (c == 0) {  // density path: d(out0) += d sigma / d raw (trunc_exp backward folded in by nsr_nerf_ray_bwd)
         if (ia < n) acc16[0][0][0] += dsr[0] * loss_scale;
         if (ib < n) acc16[0][0][2] += dsr[1] * loss_scale;
@@ -639,16 +679,14 @@ __global__ void __launch_bounds__(kNetThreads, 1) nerf_bwd_net_kernel(const __ha
       uint32_t a_do[1][1][4];
       nsr_acc_to_afrag<1, 2>(acc16, a_do, NSR_ACT_NONE);
       canon_store_afrag<1>(a_do, slot + SL_DO, 16, r0);
-      nsr_zero_acc(acc);
-      nsr_gemm_wt<1, 1, 8>(acc, a_do, W + NF_OFF_DW2, NSR_LD64);
+      chain_gemm<64, 1, 1>(acc, a_do, sbase + NW_DW2, 64);
       relu_mask_pack(acc, a_h1, a_d);
       canon_store_afrag<4>(a_d, slot + SL_DH1, 64, r0);
       // the slot is complete: make this thread's stores visible to the tensor core and hand the slot over
       nsr_proxy_fence();
       mbar_arrive(full_bar(s));
       float accE[1][4][4];
-      nsr_zero_acc(accE);
-      nsr_gemm_wt<1, 4, 4>(accE, a_d, W + NF_OFF_DW1, NF_LD32);
+      chain_gemm<32, 4, 1>(accE, a_d, sbase + NW_DW1, 32);
       // ---- d(encoding) -> fp16 pairs [n][16 levels], still multiplied by the loss scale: 4 lanes x 4 bytes = 16 contiguous bytes per (row, nt)
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {

@@ -116,3 +116,59 @@ __device__ __forceinline__ void nsr_wgmma(float (&d)[N / 2], uint64_t da, uint64
   else if constexpr (N == 32) nsr_wgmma_n32<TA, TB>(d, da, db, accumulate);
   else nsr_wgmma_n64<TA, TB>(d, da, db, accumulate);
 }
+
+// Register-A form: D[64 x N] (+)= A[64 x 16] * B[16 x N], A from registers, B from shared memory.  Each warp of the warpgroup holds
+// its 16 rows of A in the mma.sync m16n8k16 A-fragment layout (a[0]: row g, columns 2c..2c+1; a[1]: row g+8; a[2], a[3]: the same
+// rows, columns + 8); the accumulator has the layout above, which is the m16n8 C-fragment layout of each warp's 16 rows.  A registers
+// written since the last wgmma need an nsr_wg_fence in front.  TB: 0 = K-major, 1 = MN-major.
+template <int TB>
+__device__ __forceinline__ void nsr_wgmma_rs_n16(float (&d)[8], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, %14;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(TB)
+      : "memory");
+}
+
+template <int TB>
+__device__ __forceinline__ void nsr_wgmma_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "{%16, %17, %18, %19}, %20, p, 1, 1, %22;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+        "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(TB)
+      : "memory");
+}
+
+template <int TB>
+__device__ __forceinline__ void nsr_wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
+      "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+        "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+        "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+        "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(TB)
+      : "memory");
+}
+
+template <int N, int TB>
+__device__ __forceinline__ void nsr_wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  if constexpr (N == 16) nsr_wgmma_rs_n16<TB>(d, a, db, accumulate);
+  else if constexpr (N == 32) nsr_wgmma_rs_n32<TB>(d, a, db, accumulate);
+  else nsr_wgmma_rs_n64<TB>(d, a, db, accumulate);
+}
