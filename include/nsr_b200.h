@@ -407,6 +407,14 @@ int nsr_neus_field_fd_bwd(const nsr_grid_t* g, const float* points, const void* 
                           const float* b2, float radius, int32_t n_out, const float* fd_state, const float* g_out, const float* g_sdf,
                           const float* g_grad, const float* g_lap, float* grad_table, float* dW1, float* db1, float* dW2, float* db2, int64_t n,
                           const int64_t* n_dev, void* stream);
+/* nsr_neus_sdf_lattice: the SDF of the same field (centre only: nsr_neus_field_fd_fwd's sdf, bit for bit) on the planes
+ * [ix0, ix0 + n_planes) of the lattice ax f32 [nx] x ay [ny] x az [nz] (world coordinates, device): level f32 [n_planes, ny, nz]
+ * ('ij' order, z fastest), level[i][j][k] = sdf(ax[ix0 + i], ay[j], az[k]).  Only fd_state[2] (n_active) is read, so it serves the
+ * analytic field (n_active = 16, or the ProgressiveBandHashGrid level) as well: the normal type does not enter the level.
+ * Marching-cubes export of the fused SDF geometries (models/geometry.py:86-97); writes nothing but the level. */
+int nsr_neus_sdf_lattice(const nsr_grid_t* g, const float* ax, const float* ay, const float* az, int32_t nx, int32_t ny, int32_t nz,
+                         int32_t ix0, int32_t n_planes, const void* table_h, const float* W1, const float* b1, const float* W2, const float* b2,
+                         float radius, int32_t n_out, const float* fd_state, float* level, void* stream);
 /* out[0] = max(|a|, |b|, |c|) over up to three fp32 arrays (NULL / 0 skipped): the bound nsr_neus_field_bwd's amax wants. */
 int nsr_absmax3(const float* a, int64_t na, const float* b, int64_t nb, const float* c, int64_t nc, float* out, int64_t rows_cap,
                 const int64_t* rows_dev /* non-NULL: arrays are [rows_cap, w] with *rows_dev live rows */, void* stream);
@@ -505,6 +513,19 @@ int nsr_mc_count(const float* field, int32_t nx, int32_t ny, int32_t nz, float i
 int nsr_mc_emit(const float* field, int32_t nx, int32_t ny, int32_t nz, float iso, int32_t negate, const int32_t* block_offsets,
                 const float* lo, const float* hi, int32_t* vid_map, float* verts, int64_t n_verts, int64_t* faces, int64_t n_faces,
                 void* stream);
+/* The same extraction one slab of x-planes at a time (x is the slowest axis, so slabs taken in order give the dense call's vertex
+ * and face order).  The slab [a, b) (0 <= a < b <= nx) emits the vertices owned by the points with a <= ix < b and the faces of the
+ * cells whose minimum corner has a <= ix < b.  field f32 [min(b + 2, nx) - a, ny, nz] holds the planes a .. min(b + 1, nx - 1): plane
+ * b's vertex ids (faces on plane b - 1 use them) depend on its +x crossings.  With T = (b < nx ? ny*nz : 0) tail points (plane b,
+ * given ids, emitting nothing), block_offsets int32 [2 * B], B = ceil((b - a)*ny*nz / 256) + ceil(T / 256); vid_map int32
+ * [(b - a)*ny*nz + T]; totals (V, F) count the slab's own vertices and faces.  Vertex ids are slab-local (V + 3 T < 2^29 per slab);
+ * faces int64 = vbase + local id, vbase = the vertices of the slabs before.  lo / hi: the box of the WHOLE grid.
+ * nsr_mc_count / nsr_mc_emit are the slab [0, nx). */
+int nsr_mc_count_slab(const float* field, int32_t nx, int32_t ny, int32_t nz, int32_t a, int32_t b, float iso, int32_t negate,
+                      int32_t* block_offsets, int64_t* totals, void* stream);
+int nsr_mc_emit_slab(const float* field, int32_t nx, int32_t ny, int32_t nz, int32_t a, int32_t b, float iso, int32_t negate,
+                     const int32_t* block_offsets, const float* lo, const float* hi, int32_t* vid_map, float* verts, int64_t n_verts,
+                     int64_t* faces, int64_t n_faces, int64_t vbase, void* stream);
 
 /* ---- gradient exchange over NVLink peer memory (SURVEY 8e; replaces the NCCL all-reduce of Lightning DDP, launch.py:98) ---------
  * Every rank holds its flat fp32 gradient vector in a peer-mapped (symmetric) buffer of n floats (n % 4 == 0).

@@ -9,6 +9,12 @@
 // Field layout [nx, ny, nz], z fastest (torch.meshgrid(indexing='ij').reshape(-1): geometry.py:46-52).  Every pass is a coalesced
 // stream over the field (4 B/point; the +y / +x neighbour rows come from L1 / L2), i.e. HBM-bound integer work; nothing is sorted
 // and no atomics are used, so vertex and face order are deterministic.
+// Slabs: x is the slowest axis, so the planes [a, b) taken in order reproduce the dense (point, axis) vertex order and (cell, table)
+// face order.  A slab emits the vertices of the points and the faces of the cells whose x index is in [a, b); its field buffer holds
+// the planes [a, min(b + 1, nx - 1)].  The faces of cells on plane b - 1 look up vertex ids on plane b, whose +x flags read plane b + 1:
+// plane b is scanned as a TAIL after the slab's own points (its own CTAs, so the slab's vertex count is a block offset) and gets
+// vid_map entries but emits nothing.  Vertex ids in vid_map are slab-local (plane b's continue after the slab's last vertex, which is
+// where the next slab's numbering starts); faces add the 64-bit vertex base.  The dense grid is the one slab [0, nx) with no tail.
 #include "common.cuh"
 #include "mc_table.inc"
 
@@ -17,8 +23,11 @@ namespace {
 constexpr int kThreads = 256;
 
 struct McDims {
-  int32_t nx, ny, nz;
-  int64_t n;  // nx * ny * nz
+  int32_t nx, ny, nz;  // the whole grid
+  int32_t ix0;         // x index of the buffer's first plane (the slab's a)
+  int64_t n;           // the slab's own points: (b - a) * ny * nz
+  int64_t n_all;       // n + the tail plane's points (0 or ny * nz)
+  int64_t nb_main;     // CTAs over the slab's own points; the tail's CTAs follow
 };
 
 __device__ __forceinline__ float mc_value(const float* __restrict__ f, int64_t i, int negate) {
@@ -57,11 +66,23 @@ __device__ __forceinline__ void mc_point(const float* __restrict__ f, const McDi
   }
 }
 
+// buffer index of this thread's point (the slab's own points, then the tail plane's), -1 past either range
+__device__ __forceinline__ int64_t mc_index(const McDims& d) {
+  const int64_t blk = blockIdx.x;
+  if (blk < d.nb_main) {
+    const int64_t idx = blk * kThreads + threadIdx.x;
+    return idx < d.n ? idx : -1;
+  }
+  const int64_t idx = d.n + (blk - d.nb_main) * kThreads + threadIdx.x;
+  return idx < d.n_all ? idx : -1;
+}
+
+// grid coordinates of buffer index idx (ix global: the buffer starts at plane ix0)
 __device__ __forceinline__ void mc_coords(const McDims& d, int64_t idx, int& ix, int& iy, int& iz) {
   iz = (int)(idx % d.nz);
   const int64_t q = idx / d.nz;
   iy = (int)(q % d.ny);
-  ix = (int)(q / d.ny);
+  ix = (int)(q / d.ny) + d.ix0;
 }
 
 // exclusive scan of one int per thread over the 256-thread block; returns the exclusive prefix, total in `total`
@@ -90,15 +111,15 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int& total) {
 
 __global__ void __launch_bounds__(kThreads) mc_count_kernel(const float* __restrict__ f, McDims d, float iso, int negate, int32_t* __restrict__ block_v,
                                                             int32_t* __restrict__ block_t) {
-  const int64_t idx = blockIdx.x * (int64_t)kThreads + threadIdx.x;
+  const int64_t idx = mc_index(d);
   int nv = 0, nt = 0;
-  if (idx < d.n) {
+  if (idx >= 0) {
     int ix, iy, iz, vflags, cc;
     float eb[3], v0;
     mc_coords(d, idx, ix, iy, iz);
     mc_point(f, d, idx, ix, iy, iz, iso, negate, vflags, cc, eb, v0);
     nv = __popc(vflags);
-    nt = cc >= 0 ? kMcNumTris[cc] : 0;
+    nt = (cc >= 0 && idx < d.n) ? kMcNumTris[cc] : 0;  // the tail plane's cells belong to the next slab
   }
   int tv, tt;
   block_exclusive_scan(nv, tv);
@@ -107,9 +128,9 @@ __global__ void __launch_bounds__(kThreads) mc_count_kernel(const float* __restr
 }
 
 // in-place exclusive scan of two int32 arrays of n_blocks entries by ONE 1024-thread CTA (n_blocks = points / 256: 524 k at 512^3);
-// totals[0] = vertices, totals[1] = triangles
+// totals[0] = vertices before block nb_main (the slab's own; the tail plane's follow), totals[1] = triangles
 __global__ void __launch_bounds__(1024) mc_scan_kernel(int32_t* __restrict__ block_v, int32_t* __restrict__ block_t, int64_t n_blocks,
-                                                       int64_t* __restrict__ totals) {
+                                                       int64_t nb_main, int64_t* __restrict__ totals) {
   __shared__ int64_t part[2][1024];
   const int t = threadIdx.x;
   const int64_t chunk = (n_blocks + 1023) / 1024, lo = min((int64_t)t * chunk, n_blocks), hi = min(lo + chunk, n_blocks);
@@ -130,6 +151,7 @@ __global__ void __launch_bounds__(1024) mc_scan_kernel(int32_t* __restrict__ blo
   int64_t rv = part[0][t], rt = part[1][t];
   for (int64_t i = lo; i < hi; ++i) {
     const int32_t a = block_v[i], b = block_t[i];
+    if (i == nb_main) totals[0] = rv;  // a tail follows: the slab's own vertices end here
     block_v[i] = (int32_t)rv, block_t[i] = (int32_t)rt;
     rv += a, rt += b;
   }
@@ -142,17 +164,18 @@ struct McXform {
 __global__ void __launch_bounds__(kThreads) mc_vertices_kernel(const float* __restrict__ f, McDims d, float iso, int negate, McXform X,
                                                                const int32_t* __restrict__ block_v, int32_t* __restrict__ vid_map,
                                                                float* __restrict__ verts, int64_t n_verts) {
-  const int64_t idx = blockIdx.x * (int64_t)kThreads + threadIdx.x;
+  const int64_t idx = mc_index(d);
   int ix = 0, iy = 0, iz = 0, vflags = 0, cc;
   float eb[3] = {0.f, 0.f, 0.f}, v0 = 0.f;
-  if (idx < d.n) {
+  if (idx >= 0) {
     mc_coords(d, idx, ix, iy, iz);
     mc_point(f, d, idx, ix, iy, iz, iso, negate, vflags, cc, eb, v0);
   }
   int total;
   const int base = block_v[blockIdx.x] + block_exclusive_scan(__popc(vflags), total);
-  if (idx >= d.n) return;
+  if (idx < 0) return;
   vid_map[idx] = (int32_t)((uint32_t)base | ((uint32_t)vflags << 29));
+  if (idx >= d.n) return;  // tail plane: ids only, its vertices are the next slab's
   int k = 0;
   const float p[3] = {(float)ix, (float)iy, (float)iz};
 #pragma unroll
@@ -171,11 +194,11 @@ __global__ void __launch_bounds__(kThreads) mc_vertices_kernel(const float* __re
 
 __global__ void __launch_bounds__(kThreads) mc_faces_kernel(const float* __restrict__ f, McDims d, float iso, int negate,
                                                             const int32_t* __restrict__ block_t, const int32_t* __restrict__ vid_map,
-                                                            int64_t* __restrict__ faces, int64_t n_faces) {
-  const int64_t idx = blockIdx.x * (int64_t)kThreads + threadIdx.x;
+                                                            int64_t* __restrict__ faces, int64_t n_faces, int64_t vbase) {
+  const int64_t idx = mc_index(d);
   int ix = 0, iy = 0, iz = 0, vflags, cc = -1;
   float eb[3], v0;
-  if (idx < d.n) {
+  if (idx >= 0 && idx < d.n) {  // the tail's CTAs come after every face slot of the slab: no scan of theirs reaches a face
     mc_coords(d, idx, ix, iy, iz);
     mc_point(f, d, idx, ix, iy, iz, iso, negate, vflags, cc, eb, v0);
   }
@@ -194,52 +217,86 @@ __global__ void __launch_bounds__(kThreads) mc_faces_kernel(const float* __restr
       const int ox = axis == 0 ? 0 : a, oy = axis == 0 ? a : (axis == 1 ? 0 : b), oz = axis == 2 ? 0 : b;
       const uint32_t entry = (uint32_t)__ldg(vid_map + idx + ox * sx + oy * sy + oz);
       const uint32_t flags = entry >> 29;
-      faces[slot * 3 + j] = (int64_t)((entry & 0x1fffffffu) + __popc(flags & ((1u << axis) - 1u)));
+      faces[slot * 3 + j] = vbase + (int64_t)((entry & 0x1fffffffu) + __popc(flags & ((1u << axis) - 1u)));
     }
   }
 }
 
-int check_dims(const char* who, int32_t nx, int32_t ny, int32_t nz) {
+int check_dims(const char* who, int32_t nx, int32_t ny, int32_t nz, int32_t a, int32_t b) {
   NSR_REQUIRE(nx >= 2 && ny >= 2 && nz >= 2, "%s: the field needs at least 2 points per axis (got %d x %d x %d)", who, nx, ny, nz);
-  NSR_REQUIRE((int64_t)nx * ny * nz <= ((int64_t)1 << 33), "%s: field too large", who);
+  NSR_REQUIRE(0 <= a && a < b && b <= nx, "%s: plane range [%d, %d) is not a non-empty part of [0, %d)", who, a, b, nx);
+  NSR_REQUIRE((int64_t)(b - a + (b < nx)) * ny * nz <= ((int64_t)1 << 33), "%s: field too large", who);
+  return 0;
+}
+
+// the slab [a, b) of an nx x ny x nz grid (see the top of the file); *nb = CTAs of every pass (block_offsets holds 2 * nb entries)
+McDims slab_dims(int32_t nx, int32_t ny, int32_t nz, int32_t a, int32_t b, int64_t* nb) {
+  const int64_t plane = (int64_t)ny * nz, n = (b - a) * plane, tail = b < nx ? plane : 0;
+  const int64_t nb_main = (n + kThreads - 1) / kThreads;
+  *nb = nb_main + (tail + kThreads - 1) / kThreads;
+  return McDims{nx, ny, nz, a, n, n + tail, nb_main};
+}
+
+int mc_count(const char* who, const float* field, int32_t nx, int32_t ny, int32_t nz, int32_t a, int32_t b, float iso, int32_t negate,
+             int32_t* block_offsets, int64_t* totals, void* stream) {
+  if (int e = check_dims(who, nx, ny, nz, a, b)) return e;
+  NSR_REQUIRE(field != nullptr && block_offsets != nullptr && totals != nullptr, "%s: NULL argument", who);
+  int64_t nb;
+  const McDims d = slab_dims(nx, ny, nz, a, b, &nb);
+  mc_count_kernel<<<(unsigned)nb, kThreads, 0, (cudaStream_t)stream>>>(field, d, iso, negate, block_offsets, block_offsets + nb);
+  NSR_CHECK_LAUNCH(who);
+  mc_scan_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(block_offsets, block_offsets + nb, nb, d.nb_main, totals);
+  NSR_CHECK_LAUNCH(who);
+  return 0;
+}
+
+int mc_emit(const char* who, const float* field, int32_t nx, int32_t ny, int32_t nz, int32_t a, int32_t b, float iso, int32_t negate,
+            const int32_t* block_offsets, const float* lo, const float* hi, int32_t* vid_map, float* verts, int64_t n_verts, int64_t* faces,
+            int64_t n_faces, int64_t vbase, void* stream) {
+  if (int e = check_dims(who, nx, ny, nz, a, b)) return e;
+  NSR_REQUIRE(field != nullptr && block_offsets != nullptr && vid_map != nullptr, "%s: NULL argument", who);
+  NSR_REQUIRE(lo != nullptr && hi != nullptr, "%s: bounding box is NULL (host float[3] each)", who);
+  NSR_REQUIRE((n_verts == 0 || verts != nullptr) && (n_faces == 0 || faces != nullptr), "%s: output buffer is NULL", who);
+  int64_t nb;
+  const McDims d = slab_dims(nx, ny, nz, a, b, &nb);
+  // vid_map ids run on through the tail plane (at most 3 vertices per point)
+  NSR_REQUIRE(n_verts + 3 * (d.n_all - d.n) < ((int64_t)1 << 29), "%s: more than 2^29 vertices", who);
+  NSR_REQUIRE(n_faces < ((int64_t)1 << 31) && vbase >= 0, "%s: more than 2^31 faces or a negative vertex base", who);
+  McXform X;
+  const int32_t dims[3] = {nx, ny, nz};
+  for (int c = 0; c < 3; ++c) X.lo[c] = lo[c], X.ext[c] = hi[c] - lo[c], X.denom[c] = (float)(dims[c] - 1);
+  mc_vertices_kernel<<<(unsigned)nb, kThreads, 0, (cudaStream_t)stream>>>(field, d, iso, negate, X, block_offsets, vid_map, verts, n_verts);
+  NSR_CHECK_LAUNCH(who);
+  if (n_faces > 0) {
+    mc_faces_kernel<<<(unsigned)nb, kThreads, 0, (cudaStream_t)stream>>>(field, d, iso, negate, block_offsets + nb, vid_map, faces, n_faces,
+                                                                        vbase);
+    NSR_CHECK_LAUNCH(who);
+  }
   return 0;
 }
 
 }  // namespace
 
-static int64_t mc_num_blocks(int32_t nx, int32_t ny, int32_t nz) { return ((int64_t)nx * ny * nz + kThreads - 1) / kThreads; }
-
 extern "C" int nsr_mc_count(const float* field, int32_t nx, int32_t ny, int32_t nz, float iso, int32_t negate, int32_t* block_offsets,
                             int64_t* totals, void* stream) {
-  if (int e = check_dims("nsr_mc_count", nx, ny, nz)) return e;
-  NSR_REQUIRE(field != nullptr && block_offsets != nullptr && totals != nullptr, "nsr_mc_count: NULL argument");
-  const McDims d{nx, ny, nz, (int64_t)nx * ny * nz};
-  const int64_t nb = mc_num_blocks(nx, ny, nz);
-  mc_count_kernel<<<(unsigned)nb, kThreads, 0, (cudaStream_t)stream>>>(field, d, iso, negate, block_offsets, block_offsets + nb);
-  NSR_CHECK_LAUNCH("nsr_mc_count");
-  mc_scan_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(block_offsets, block_offsets + nb, nb, totals);
-  NSR_CHECK_LAUNCH("nsr_mc_count (scan)");
-  return 0;
+  return mc_count("nsr_mc_count", field, nx, ny, nz, 0, nx, iso, negate, block_offsets, totals, stream);
 }
 
 extern "C" int nsr_mc_emit(const float* field, int32_t nx, int32_t ny, int32_t nz, float iso, int32_t negate, const int32_t* block_offsets,
                            const float* lo, const float* hi, int32_t* vid_map, float* verts, int64_t n_verts, int64_t* faces,
                            int64_t n_faces, void* stream) {
-  if (int e = check_dims("nsr_mc_emit", nx, ny, nz)) return e;
-  NSR_REQUIRE(field != nullptr && block_offsets != nullptr && vid_map != nullptr, "nsr_mc_emit: NULL argument");
-  NSR_REQUIRE(lo != nullptr && hi != nullptr, "nsr_mc_emit: bounding box is NULL (host float[3] each)");
-  NSR_REQUIRE((n_verts == 0 || verts != nullptr) && (n_faces == 0 || faces != nullptr), "nsr_mc_emit: output buffer is NULL");
-  NSR_REQUIRE(n_verts < ((int64_t)1 << 29), "nsr_mc_emit: more than 2^29 vertices");
-  const McDims d{nx, ny, nz, (int64_t)nx * ny * nz};
-  const int64_t nb = mc_num_blocks(nx, ny, nz);
-  McXform X;
-  const int32_t dims[3] = {nx, ny, nz};
-  for (int c = 0; c < 3; ++c) X.lo[c] = lo[c], X.ext[c] = hi[c] - lo[c], X.denom[c] = (float)(dims[c] - 1);
-  mc_vertices_kernel<<<(unsigned)nb, kThreads, 0, (cudaStream_t)stream>>>(field, d, iso, negate, X, block_offsets, vid_map, verts, n_verts);
-  NSR_CHECK_LAUNCH("nsr_mc_emit (vertices)");
-  if (n_faces > 0) {
-    mc_faces_kernel<<<(unsigned)nb, kThreads, 0, (cudaStream_t)stream>>>(field, d, iso, negate, block_offsets + nb, vid_map, faces, n_faces);
-    NSR_CHECK_LAUNCH("nsr_mc_emit (faces)");
-  }
-  return 0;
+  return mc_emit("nsr_mc_emit", field, nx, ny, nz, 0, nx, iso, negate, block_offsets, lo, hi, vid_map, verts, n_verts, faces, n_faces, 0,
+                 stream);
+}
+
+extern "C" int nsr_mc_count_slab(const float* field, int32_t nx, int32_t ny, int32_t nz, int32_t a, int32_t b, float iso, int32_t negate,
+                                 int32_t* block_offsets, int64_t* totals, void* stream) {
+  return mc_count("nsr_mc_count_slab", field, nx, ny, nz, a, b, iso, negate, block_offsets, totals, stream);
+}
+
+extern "C" int nsr_mc_emit_slab(const float* field, int32_t nx, int32_t ny, int32_t nz, int32_t a, int32_t b, float iso, int32_t negate,
+                                const int32_t* block_offsets, const float* lo, const float* hi, int32_t* vid_map, float* verts,
+                                int64_t n_verts, int64_t* faces, int64_t n_faces, int64_t vbase, void* stream) {
+  return mc_emit("nsr_mc_emit_slab", field, nx, ny, nz, a, b, iso, negate, block_offsets, lo, hi, vid_map, verts, n_verts, faces, n_faces,
+                 vbase, stream);
 }

@@ -103,6 +103,7 @@ _SIGNATURES = {
     'nsr_neus_field_bwd_levels': [P, P, P, P, P, P, P, F32, I32, P, P, P, P, P, P, P, P, P, P, I64, P, P],
     'nsr_neus_field_fd_fwd': [P, P, P, P, P, P, P, F32, I32, P, P, P, P, P, I64, P, P],
     'nsr_neus_field_fd_bwd': [P, P, P, P, P, P, P, F32, I32, P, P, P, P, P, P, P, P, P, P, I64, P, P],
+    'nsr_neus_sdf_lattice': [P, P, P, P, I32, I32, I32, I32, I32, P, P, P, P, P, F32, I32, P, P, P],
     'nsr_absmax3': [P, I64, P, I64, P, I64, P, I64, P, P],
     'nsr_sample_points': [P, P, P, P, P, P, P, I64, P, P],
     'nsr_neus_alpha_fwd': [P, P, P, P, P, F32, P, P, P, I64, P, P],
@@ -131,6 +132,8 @@ _SIGNATURES = {
     'nsr_gather_rays': [P, I32, P, I32, P, I32, P, P, P, P, I32, P, I32, I32, I32, I32, P, P, P, I64, P],
     'nsr_mc_count': [P, I32, I32, I32, F32, I32, P, P, P],
     'nsr_mc_emit': [P, I32, I32, I32, F32, I32, P, P, P, P, P, I64, P, I64, P],
+    'nsr_mc_count_slab': [P, I32, I32, I32, I32, I32, F32, I32, P, P, P],
+    'nsr_mc_emit_slab': [P, I32, I32, I32, I32, I32, F32, I32, P, P, P, P, P, I64, P, I64, I64, P],
     'nsr_nerf_density': [P, P, P, P, I64, P],
     'nsr_nerf_prepass': [P, P, P, P, P, P, P, I64, P, P],
     'nsr_compact_prefix': [P, P, P, P, P, P, P, P, P, P, I64, P],
@@ -203,7 +206,8 @@ lib = _Lib()
 
 
 # entry points that launch more than one kernel (lib.launches counts kernels, not calls)
-_KERNELS_PER_CALL = {'nsr_nerf_field_bwd_split': 2, 'nsr_nerf_loss_fwd': 2, 'nsr_neus_loss_fwd': 2, 'nsr_distortion_fwd': 2, 'nsr_occgrid_update': 2, 'nsr_mc_count': 2, 'nsr_mc_emit': 2}
+_KERNELS_PER_CALL = {'nsr_nerf_field_bwd_split': 2, 'nsr_nerf_loss_fwd': 2, 'nsr_neus_loss_fwd': 2, 'nsr_distortion_fwd': 2, 'nsr_occgrid_update': 2, 'nsr_mc_count': 2, 'nsr_mc_emit': 2,
+                     'nsr_mc_count_slab': 2, 'nsr_mc_emit_slab': 2}
 
 
 def register_signatures(sigs):

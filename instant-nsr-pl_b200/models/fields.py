@@ -40,14 +40,28 @@ class BaseImplicitGeometry(BaseModel):
     def forward_level(self, points):
         raise NotImplementedError
 
+    def fused_level_unsupported(self):
+        """None when isosurface.fused evaluates this field's level with a lattice kernel, else why it streams through forward_level"""
+        return f'{type(self).__name__} has no lattice kernel: its level streams through forward_level'
+
+    def _level_planes(self, chunk):
+        """level_planes(axes, a, b, out) for mcubes.isosurface_slabs"""
+        from .. import mcubes
+        return mcubes.forward_level_planes(self.forward_level, chunk)
+
     @torch.no_grad()
     def isosurface(self):
-        """models/geometry.py:80-112: coarse + refined marching cubes over the level field, here extracted on the GPU (nsr_b200.mcubes)"""
+        """models/geometry.py:80-112: coarse + refined marching cubes over the level field, here extracted on the GPU (nsr_b200.mcubes).
+        With ``isosurface.fused: true`` both passes stream over slabs of ``isosurface.slab`` x-planes (default 64), the level of a fused
+        SDF geometry coming from its lattice kernel (fused_level_unsupported() says why another geometry uses forward_level)."""
         iso = self.config.get('isosurface', None)
         if iso is None:
             raise NotImplementedError
         from .. import mcubes
         device = next(self.parameters()).device
+        if iso.get('fused', False):
+            return mcubes.isosurface_slabs(self._level_planes(iso.chunk), self.radius, iso.resolution, iso.threshold, iso.get('slab', 64),
+                                           device)
         return mcubes.isosurface(self.forward_level, self.radius, iso.resolution, iso.threshold, iso.chunk, device)
 
 
@@ -163,6 +177,31 @@ class VolumeSDF(BaseImplicitGeometry):
         if self.n_output_dims != 13:
             return f'the colour input is [feature 13 | SH4 | normal]: feature_dim is {self.n_output_dims}'
         return None
+
+    def fused_level_unsupported(self):
+        """None when isosurface.fused evaluates the level with the lattice kernel (ops.neus_sdf_lattice: the fused SDF field shapes,
+        analytic or finite-difference), else why the level streams through forward_level (a message)."""
+        if not self.config.get('fused', True):
+            return 'the geometry runs the per-op path (fused: false): its level streams through forward_level'
+        if not (self._fused or self._fused_fd):
+            if self._progressive and self.grad_type == 'analytic' and not self.config.get('fused_progressive', False):
+                return 'a ProgressiveBandHashGrid runs the fused field only with fused_progressive: true'
+            return ('the geometry is not a fused SDF field shape (include_xyz HashGrid or ProgressiveBandHashGrid L=16 F=2 + sphere-init '
+                    'VanillaMLP 35 -> 64 -> n_out <= 16): its level streams through forward_level')
+        if self.contraction_type != ContractionType.AABB:
+            return f'the lattice kernel maps world points to the unit cube by the AABB contraction, the field uses {self.contraction_type}'
+        return None
+
+    def _level_planes(self, chunk):
+        if self.fused_level_unsupported() is not None:
+            return super()._level_planes(chunk)
+        enc = self._fd_grid()
+        W1, b1, W2, b2 = self._effective_weights()
+        table_h = enc._params_half()
+
+        def planes(axes, a, b, out):
+            ops.neus_sdf_lattice(enc.grid, self.radius, axes, a, b, table_h, W1, b1, W2, b2, self._fd_state, out)
+        return planes
 
     def _n_active_levels(self):
         return int(self.encoding.encoding.current_level) if self._progressive else 16

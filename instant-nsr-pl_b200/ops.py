@@ -630,6 +630,25 @@ def neus_sdf_fd(spec, radius, points, table_f32, table_h, W1, b1, W2, b2, fd_sta
                             fd_state)
 
 
+def neus_sdf_lattice(spec, radius, axes, a, b, table_h, W1, b1, W2, b2, fd_state, out):
+    """the SDF of the fused NeuS field (the centre value of neus_sdf_fd; neus_sdf's field under the same level mask) on the x-planes
+    [a, b) of the lattice axes[0] x axes[1] x axes[2] (world coordinates, CUDA fp32 vectors) into out fp32 [b - a, ny, nz]
+    ('ij' order).  fd_state: VolumeSDF._fd_state (only n_active = fd_state[2] is read)."""
+    ax, ay, az = (contig(t, torch.float32) for t in axes)
+    check_cuda(ax, ay, az, table_h, W1, W2, fd_state, out, what='neus_sdf_lattice')
+    if fd_state.dtype != torch.float32 or fd_state.numel() != 3 or not fd_state.is_contiguous():
+        raise ValueError('fd_state must be a contiguous float32 tensor of 3 entries {eps, eps^2, n_active}')
+    nx, ny, nz = ax.numel(), ay.numel(), az.numel()
+    if out.dtype != torch.float32 or not out.is_contiguous() or tuple(out.shape) != (b - a, ny, nz):
+        raise ValueError(f'neus_sdf_lattice: out must be a contiguous float32 [{b - a}, {ny}, {nz}] tensor, got {out.dtype} {tuple(out.shape)}')
+    if b <= a:
+        return out
+    lib.call('nsr_neus_sdf_lattice', spec.ref(), ptr(ax), ptr(ay), ptr(az), nx, ny, nz, int(a), int(b - a), ptr(table_h), ptr(contig(W1, torch.float32)),
+             ptr(contig(b1, torch.float32)), ptr(contig(W2, torch.float32)), ptr(contig(b2, torch.float32)), float(radius), int(W2.shape[0]),
+             ptr(fd_state), ptr(out), stream())
+    return out
+
+
 # --------------------------------------------------------------------------------------------------
 # NeuS shading: SDF -> alpha (+ normal), compositing, fused VolumeRadiance
 # --------------------------------------------------------------------------------------------------
