@@ -1,5 +1,8 @@
 """Plain fp64 restatement of the fused NeRF field backward (nsr_nerf_field_bwd / _split / _net + nsr_nerf_table_scatter / _tc) on the
-packed inputs, an entry-by-entry error scale, and the checker the kernel tests use.
+packed inputs, an entry-by-entry error scale, and the checker the kernel tests use.  With fp32 biases (split_params' dbias / cbias) it
+is the VanillaMLP field of nsr_bg_field_bwd: every layer starts from its bias, the colour sigmoid acts on the un-rounded raw, and the
+bias gradients are the column sums of the five pre-activation-gradient tiles (see bias_rtol for their summation bound).  The colour
+network is radiance_ref's restatement (forward / backward of the 32 -> 64 -> 64 -> 16 net), fed with [out16 | SH4].
 
 The forward is recomputed from the saved fp16 encodings and rounded to fp16 exactly where the kernels round (H1, out16, SH4, G1, G2,
 rgb_raw); the ReLU masks come from those fp16 activations.  The backward is fp64 with no rounding.  Its outputs: the five weight
@@ -30,13 +33,37 @@ TIE_ROW_LIMIT = 1e-3
 N_DENSITY = 64 * 32 + 16 * 64          # DW1 [64][32], DW2 [16][64]; the table follows in the flat density parameters
 N_COLOR = 64 * 32 + 64 * 64 + 16 * 64  # CW1 [64][32], CW2 [64][64], CW3 [16][64] (rows 3..15 padding)
 ACC_REL = 2.0 ** -23                   # the kernels' fp32 accumulation error (K <= 64 exact products), relative to the sum's absolute mass
+RAW_ACC = 2.0 ** -16                   # VanillaMLP raw colour: fp32 accumulation plus the fp16 flips of G2 it can carry, relative to its mass
+RTOL_OUT = 2.0 ** -10                  # dC3-only gradients (dCW3, colour output bias): one fp16 rounding and the fp32 sigmoid', as radiance_ref
+EPS32 = 2.0 ** -24
 SH_ABS = 2.0 ** -22                    # fp32 SH4 evaluation error (fma contraction on the device, none here)
 
 
-def split_params(dparams16, cparams16):
+def split_params(dparams16, cparams16, dbias=None, cbias=None):
+    """weights by layer; dbias [80] / cbias [144] (VanillaMLP, fp32, padded as ops.pack_background_field pads them): the biases
+    DB1 [64], DB2 [16], CB1 [64], CB2 [64], CB3 [16]"""
     d, c = dparams16, cparams16
-    return {'DW1': d[:2048].view(64, 32), 'DW2': d[2048:3072].view(16, 64),
-            'CW1': c[:2048].view(64, 32), 'CW2': c[2048:6144].view(64, 64), 'CW3': c[6144:7168].view(16, 64)}
+    W = {'DW1': d[:2048].view(64, 32), 'DW2': d[2048:3072].view(16, 64),
+         'CW1': c[:2048].view(64, 32), 'CW2': c[2048:6144].view(64, 64), 'CW3': c[6144:7168].view(16, 64)}
+    if dbias is not None:
+        W.update(DB1=dbias[:64], DB2=dbias[64:80], CB1=cbias[:64], CB2=cbias[64:128], CB3=cbias[128:144])
+    return W
+
+
+def colour_weights(W):
+    """the colour network's layers in radiance_ref's naming (biases None without them)"""
+    return dict(W1=W['CW1'], W2=W['CW2'], W3=W['CW3'], b1=W.get('CB1'), b2=W.get('CB2'), b3=W.get('CB3'))
+
+
+def bias_rtol(k, n_ctas, rows=64):
+    """rtol of the VanillaMLP bias gradients.  Each is a sum over k rows of fp16 tile entries, taken by the kernel as: a sequential
+    fp32 sum of the 64 rows of one tile (each add loses at most 2^-24 of the running sum's absolute mass), then tiles_per_CTA adds of
+    those into the thread's register (the same, per add), then one atomicAdd per CTA into the gradient (n_CTAs adds); the loss-scale
+    division is exact.  Every partial sum's mass is at most the column's sum of |terms|, which M bounds, so the fp32 summation adds
+    (64 + tiles_per_CTA + n_CTAs) * 2^-24 * M to the fp16 rounding of the tiles (RTOL * M)."""
+    tiles = -(-k // rows)
+    n = max(1, min(n_ctas, tiles))
+    return RTOL + (rows + -(-tiles // n) + n) * 2.0 ** -24
 
 
 def auto_loss_scale(amax):
@@ -75,22 +102,25 @@ def _mid_dist(pre):
     return _ulp16(pre) * 0.5 - (pre - _r16(pre)).abs()
 
 
+def _lin(x, w, b):
+    return x @ w.T if b is None else x @ w.T + b
+
+
 def forward(enc16, dirs, W, dtype):
-    """fp16-rounded activations of the kernels' forward recompute, evaluated in `dtype`"""
+    """fp16-rounded activations of the kernels' forward recompute, evaluated in `dtype`.  o: the density output before its fp16
+    rounding (VanillaMLP's sigma comes from it); raw: the colour output before the fp16 rounding FullyFused applies; s: the sigmoid"""
+    from helpers import radiance_ref as rr
     E = enc16.to(dtype)
     Wd = {k: v.to(dtype) for k, v in W.items()}
-    h1 = E @ Wd['DW1'].T
+    h1 = _lin(E, Wd['DW1'], Wd.get('DB1'))
     H1 = _r16(h1).clamp_min(0)
-    O = _r16(H1 @ Wd['DW2'].T)
+    o = _lin(H1, Wd['DW2'], Wd.get('DB2'))
+    O = _r16(o)
     sh32 = sh4_f32(dirs)
     CI = torch.cat([O, _r16(sh32.to(dtype))], 1)
-    g1 = CI @ Wd['CW1'].T
-    G1 = _r16(g1).clamp_min(0)
-    g2 = G1 @ Wd['CW2'].T
-    G2 = _r16(g2).clamp_min(0)
-    raw = _r16((G2 @ Wd['CW3'].T)[:, :3])
-    s = torch.sigmoid(raw.float()).to(dtype)   # the kernels: 1 / (1 + expf(-raw)) in fp32
-    return dict(E=E, H1=H1, O=O, CI=CI, G1=G1, G2=G2, s=s, pre=dict(h1=h1, g1=g1, g2=g2), sh32=sh32)
+    C = rr.forward(CI, colour_weights(W), 2, 'CB1' in W, dtype)
+    s = torch.sigmoid(C['used'].float()).to(dtype)   # the kernels: 1 / (1 + expf(-raw)) in fp32
+    return dict(E=E, H1=H1, o=o, O=O, CI=CI, G1=C['H1'], G2=C['H2'], raw=C['raw'], s=s, pre=dict(h1=h1, g1=C['h1'], g2=C['h2']), sh32=sh32)
 
 
 def _act_perturbation(pre, live, tie, bnd, acc):
@@ -135,38 +165,43 @@ def _tie_masks(A, W):
     """per pre-activation: can the kernel's ReLU decision differ from ours?  The bound on |kernel pre - our pre| is the fp32
     accumulation error plus the fp16 rounding flips it allows upstream, propagated layer by layer."""
     E = A['E'].double()
-    (tie_h1,), _ = relu_ties(E, torch.zeros_like(E), [(A['pre']['h1'], W['DW1'], None, A['H1'])])
+    (tie_h1,), _ = relu_ties(E, torch.zeros_like(E), [(A['pre']['h1'], W['DW1'], W.get('DB1'), A['H1'])])
     H1 = A['H1'].double()
-    o = H1 @ W['DW2'].double().T
-    p_o = _ulp16(o) * (_mid_dist(o) <= ACC_REL * (H1 @ W['DW2'].double().abs().T))
+    o = A['o'].double()
+    db2 = 0.0 if W.get('DB2') is None else W['DB2'].double().abs()
+    p_o = _ulp16(o) * (_mid_dist(o) <= ACC_REL * (H1 @ W['DW2'].double().abs().T + db2))
     sh = A['sh32'].double()
     p_sh = _ulp16(sh) * (_mid_dist(sh) <= SH_ABS)
     ties, _ = relu_ties(A['CI'], torch.cat([p_o, p_sh], 1),
-                        [(A['pre']['g1'], W['CW1'], None, A['G1']), (A['pre']['g2'], W['CW2'], None, A['G2'])])
+                        [(A['pre']['g1'], W['CW1'], W.get('CB1'), A['G1']), (A['pre']['g2'], W['CW2'], W.get('CB2'), A['G2'])])
     return [tie_h1] + ties
 
 
 def backward(W, A, masks, dc3, dsr, ls, dtype, store=None, inject=0.0):
     """dgrad + wgrad chain on loss-scaled gradients (what the kernels carry); returns unscaled results.
-    store(x): applied where the kernels store an fp16 gradient; inject: added there (the floor pass)."""
+    store(x): applied where the kernels store an fp16 gradient; inject: added there (the floor pass).
+    The colour half is radiance_ref.backward on the input [out16 | SH4] (its d_feat: the first 16 columns of d(input)).  With biases
+    in W also dbias [80] / cbias [144] (column sums of [dH1 | dO] and [dG1 | dG2 | dC3]) and the five loss-scaled fp16 tiles."""
+    from helpers import radiance_ref as rr
     st = store or (lambda x: x)
     Wd = {k: v.to(dtype) for k, v in W.items()}
-    m_h1, m_g1, m_g2 = (m.to(dtype) for m in masks)
+    m_h1 = masks[0].to(dtype)
     n = dc3.shape[0]
-    dC3 = st(dc3.to(dtype) * ls + inject)                                # [n, 3]
-    dG2 = st((dC3 @ Wd['CW3'][:3]) * m_g2 + inject * m_g2)
-    dG1 = st((dG2 @ Wd['CW2']) * m_g1 + inject * m_g1)
-    dO = (dG1 @ Wd['CW1'][:, :16])
+    C = rr.backward(colour_weights(W), dict(X=A['CI'], H1=A['G1'], H2=A['G2']), masks[1:], dc3, ls, 16, 0, dtype, store=store,
+                    inject=inject)
+    dO = C['d_feat'] * ls
     dO[:, 0] += dsr.to(dtype) * ls
     dO = st(dO + inject)
     dH1 = st((dO @ Wd['DW2']) * m_h1 + inject * m_h1)
     dE = st(dH1 @ Wd['DW1'] + inject)
-    dCW3 = torch.zeros(16, 64, dtype=dtype, device=dC3.device)
-    dCW3[:3] = dC3.T @ A['G2'].to(dtype)
     gd_net = torch.cat([(dH1.T @ A['E'].to(dtype)).flatten(), (dO.T @ A['H1'].to(dtype)).flatten()]) / ls
-    gc = torch.cat([(dG1.T @ A['CI'].to(dtype)).flatten(), (dG2.T @ A['G1'].to(dtype)).flatten(), dCW3.flatten()]) / ls
-    scaled_max = max(float(t.abs().max()) if n else 0.0 for t in (dC3, dG2, dG1, dO, dH1, dE))
-    return dict(gd_net=gd_net, gc=gc, denc=dE / ls, scaled_max=scaled_max)
+    scaled_max = max([C['scaled_max']] + [float(t.abs().max()) if n else 0.0 for t in (dO, dH1, dE)])
+    out = dict(gd_net=gd_net, gc=C['params'], denc=dE / ls, scaled_max=scaled_max)
+    if 'DB1' in W:
+        t = C['tiles']
+        out.update(dbias=torch.cat([dH1.sum(0), dO.sum(0)]) / ls, cbias=C['bias'],
+                   tiles=dict(dH1=dH1, dO=dO, dG1=t['dG1'], dG2=t['dG2'], dC3=t['D3']))
+    return out
 
 
 def level_geometry(xyz, lt, l):
@@ -224,12 +259,15 @@ def rows_touching(xyz, lt, entries):
     return hit.nonzero().flatten().tolist()
 
 
-def field_bwd_reference(enc16, xyzdir, d_sraw, d_rgb, dparams16, cparams16, lt, loss_scale):
+def field_bwd_reference(enc16, xyzdir, d_sraw, d_rgb, dparams16, cparams16, lt, loss_scale, dbias=None, cbias=None):
     """fp64 reference + error scale + floor of the field backward on k packed rows.  Returns a dict of 'ref', 'M', 'floor'
-    (each with 'gd_net' [3072], 'gc' [7168], 'denc' [k, 32], 'table' [entries * 2]), 'tie_rows', 'scaled_max' (largest |loss-scaled
-    stored gradient|, the fp16 headroom of the dgrad chain) and 'loss_scale'."""
+    (each with 'gd_net' [3072], 'gc' [7168], 'denc' [k, 32], 'table' [entries * 2]; with biases also 'dbias' [80], 'cbias' [144]),
+    'tie_rows', 'scaled_max' (largest |loss-scaled stored gradient|, the fp16 headroom of the dgrad chain) and 'loss_scale'.
+    xyzdir: the unit-cube position the table gradient is scattered at (the contracted one for the background field) and the view
+    direction.  VanillaMLP: the kernel's fp32 sigmoid' of its fp32 raw (radiance_ref's widening: raw may be off by the accumulation
+    error, and 1 / (1 + expf(-raw)) carries ~2^-24 absolute) widens M of everything downstream of dC3."""
     k = enc16.shape[0]
-    W = split_params(dparams16, cparams16)
+    W = split_params(dparams16, cparams16, dbias, cbias)
     xyz, dirs = xyzdir[:, :3].float(), xyzdir[:, 3:6].float()
     f64 = torch.float64
     A = forward(enc16, dirs, W, f64)
@@ -248,12 +286,18 @@ def field_bwd_reference(enc16, xyzdir, d_sraw, d_rgb, dparams16, cparams16, lt, 
     Aa = dict(A, E=A['E'].abs(), CI=A['CI'].abs())
     open_masks = [m | t for m, t in zip(masks, ties)]
     wrow = 1.0 + (2.0 / RTOL) * tie_rows.double()
-    M = backward(Wa, Aa, open_masks, dc3.abs() * wrow[:, None], dsr.abs() * wrow, loss_scale, f64)
+    m3 = dc3.abs()
+    if dbias is not None:
+        mass = A['G2'].double() @ W['CW3'].double().abs()[:3].T + W['CB3'].double().abs()[:3]
+        e3 = drgb.abs() * (m3 * (1 - 2 * sg).abs() * RAW_ACC * mass + 4 * EPS32)
+        m3 = m3 + e3 / RTOL_OUT
+    M = backward(Wa, Aa, open_masks, m3 * wrow[:, None], dsr.abs() * wrow, loss_scale, f64)
     fl = backward(Wa, Aa, open_masks, torch.zeros_like(dc3), torch.zeros_like(dsr), loss_scale, f64, inject=2.0 ** -24)
     for part in (ref, M, fl):
         part['table'] = table_grad(xyz, part['denc'], lt, f64)
+    keys = ('gd_net', 'gc', 'denc', 'table') + (('dbias', 'cbias') if dbias is not None else ())
     for part in (M, fl):
-        for key in ('gd_net', 'gc', 'denc', 'table'):
+        for key in keys:
             part[key] = part[key].abs()
     return dict(ref=ref, M=M, floor=fl, tie_rows=tie_rows, scaled_max=ref['scaled_max'], loss_scale=loss_scale, xyz=xyz, lt=lt)
 
@@ -277,6 +321,8 @@ def field_bwd_standin(enc16, xyzdir, d_sraw, d_rgb, dparams16, cparams16, lt, lo
 def check(got, ref, M, rtol=RTOL, floor=0.0, what='', rows_of=None, n_worst=6):
     """assert |got - ref| <= rtol * M + floor entrywise (NaN fails); returns the worst |error| / bound (the headroom)"""
     got, ref = got.double().flatten(), ref.double().flatten().to(got.device)
+    if torch.is_tensor(rtol):
+        rtol = rtol.double().flatten().to(got.device)
     bound = rtol * M.double().flatten().to(got.device) + (floor.double().flatten().to(got.device) if torch.is_tensor(floor) else floor)
     err = (got - ref).abs()
     ok = err <= bound
@@ -286,7 +332,7 @@ def check(got, ref, M, rtol=RTOL, floor=0.0, what='', rows_of=None, n_worst=6):
     if not bool(ok.all()):
         n_bad = int((~ok).sum())
         idx = torch.topk(ratio, min(n_worst, ratio.numel())).indices.tolist()
-        lines = [f'{what}: {n_bad} of {got.numel()} entries outside rtol * M + floor (rtol {rtol:g}); worst:']
+        lines = [f'{what}: {n_bad} of {got.numel()} entries outside rtol * M + floor (rtol {float(rtol.max()) if torch.is_tensor(rtol) else rtol:g}); worst:']
         for i in idx:
             lines.append(f'  [{i}] got {float(got[i]):.6e} ref {float(ref[i]):.6e} |err| {float(err[i]):.3e} bound {float(bound[i]):.3e}')
         if rows_of is not None:
@@ -295,24 +341,36 @@ def check(got, ref, M, rtol=RTOL, floor=0.0, what='', rows_of=None, n_worst=6):
     return worst
 
 
-def check_all(got, R, what='', rtol=RTOL, parts=('gd_net', 'gc', 'table'), prefill=None):
+def check_all(got, R, what='', rtol=RTOL, parts=('gd_net', 'gc', 'table'), prefill=None, n_ctas=None):
     """check the parts of a backward result against field_bwd_reference's R; prefill: the values the gradient buffers held
-    before the call (the kernels accumulate).  Returns {part: headroom}."""
+    before the call (the kernels accumulate).  n_ctas: the VanillaMLP backward's grid, for the bias gradients' summation bound
+    (bias_rtol); their last-layer entries (cbias 128..143, one fp16 rounding of dC3 as in radiance_ref) and those of dCW3 are held
+    to RTOL_OUT.  Returns {part: headroom}."""
     out = {}
+    k = R['xyz'].shape[0]
     for p in parts:
-        g = got[p].double()
+        g = got[p].double().flatten()
         extra = 0.0
         if prefill is not None and p in prefill:
             pf = prefill[p].double().flatten().to(g.device)
-            g = g.flatten() - pf
+            g = g - pf
             extra = 2.0 ** -23 * pf.abs()   # fp32 rounding of prefill + gradient
         rows_of = None
         if p == 'table':
             rows_of = lambda idx: rows_touching(R['xyz'], R['lt'], idx)
         elif p == 'denc':
             rows_of = lambda idx: sorted({i // 32 for i in idx})
+        rt = rtol
+        if 'dbias' in R['ref']:
+            if p in ('dbias', 'cbias'):
+                rt = torch.full((g.numel(),), bias_rtol(k, n_ctas), dtype=torch.float64, device=g.device)
+                if p == 'cbias':
+                    rt[128:] = RTOL_OUT + bias_rtol(k, n_ctas) - RTOL
+            elif p == 'gc':
+                rt = torch.full((g.numel(),), rtol, dtype=torch.float64, device=g.device)
+                rt[6144:] = RTOL_OUT
         fl = R['floor'][p].to(g.device)
-        out[p] = check(g, R['ref'][p], R['M'][p].to(g.device), rtol, fl + extra if torch.is_tensor(extra) else fl, f'{what} {p}', rows_of)
+        out[p] = check(g, R['ref'][p], R['M'][p].to(g.device), rt, fl + extra if torch.is_tensor(extra) else fl, f'{what} {p}', rows_of)
     return out
 
 

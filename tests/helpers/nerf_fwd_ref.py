@@ -10,7 +10,8 @@ downstream:
   2  encoding: trilinear interpolation of the fp16 table in fp64 with the kernels' fp32 cells and corner weights, rounded to fp16 --
      bit for bit, except one fp16 ulp where the fp64 value lies within the fp32 accumulation bound of a rounding midpoint;
   3  networks: field_bwd_ref.forward in fp64 from the kernel's encodings, sigma = exp(out16[0] + density_bias), rgb = sigmoid(raw);
-     scale: the fp32 exp / sigmoid error plus the fp16 flips an fp32 accumulation can cause, propagated layer by layer;
+     scale: the fp32 exp / sigmoid error plus the fp16 flips an fp32 accumulation can cause, propagated layer by layer (VanillaMLP, the
+     background field: biases, sigma from the un-rounded out[0], rgb from the un-rounded raw -- see field());
   4  compositing: alpha, exclusive T, w and the per-ray sums in fp64 from the kernel's sigmas / rgbs; T's scale grows with the sample
      index (one fp32 rounding per factor) plus the alpha errors, the sums' with their absolute mass;
   5  kept decision: one-sided -- every kept sample has T_ref + b >= eps, the first dropped one T_ref - b < eps.  T of the first dropped
@@ -126,51 +127,58 @@ def _flip(pre, bnd):
 
 def field(enc16, dirs, W, density_bias, p_enc=None, sh_fault=False, dtype=torch.float64):
     """the networks on the given fp16 encodings: sigma, rgb and their error scales M_sigma, M_rgb, and the tie rows (a ReLU decision
-    inside the bound).  p_enc: per-entry perturbation of the encodings (nsr_nerf_density has no stored encodings to start from)."""
+    inside the bound).  p_enc: per-entry perturbation of the encodings (nsr_nerf_density has no stored encodings to start from).
+    W with biases (field_bwd_ref.split_params' dbias / cbias): the VanillaMLP field of nsr_bg_field_*.  Every accumulation then starts
+    from its fp32 bias (|bias| counts in the mass), sigma = exp(out0 + density_bias) takes the un-rounded fp32 output (its scale is the
+    accumulation bound, no fp16 flip), the colour network the fp16-rounded one, and rgb = sigmoid of the un-rounded fp32 raw."""
+    vanilla = 'DB1' in W
     dirs = torch.as_tensor(np.asarray(dirs, F32))
     if sh_fault:
         dirs = (dirs + 1) * 0.5
     A = fb.forward(torch.as_tensor(enc16).cpu(), dirs, W, dtype)
-    x = A['O'][:, 0].double() + float(F32(density_bias))
+    out0 = (A['o'] if vanilla else A['O'])[:, 0]
+    x = out0.double() + float(F32(density_bias))
     sigma = torch.exp(x)
     rgb = A['s'].double()
     if dtype != torch.float64:
         return sigma, rgb
     Wa = {k: v.double().abs() for k, v in W.items()}
+    ba = lambda key: Wa[key] if vanilla else 0.0
     E = A['E'].abs()
     pE = torch.zeros_like(E) if p_enc is None else p_enc.double()
     # density layer 1 (ReLU) and the fp16 network output
     prop = pE @ Wa['DW1'].T
-    bnd = NET_ACC * (E @ Wa['DW1'].T) + prop
+    bnd = NET_ACC * (E @ Wa['DW1'].T + ba('DB1')) + prop
     h1 = A['pre']['h1']
     tie_h1 = (h1.abs() <= bnd) & (bnd > 0)
     live = A['H1'] > 0
     p_h1 = torch.where(live | tie_h1, _flip(h1, bnd) + prop, torch.zeros_like(h1)) + torch.where(tie_h1, h1.abs() + bnd, torch.zeros_like(h1))
-    o = A['H1'] @ W['DW2'].double().T
+    o = A['o'].double()
     prop = p_h1 @ Wa['DW2'].T
-    bnd = NET_ACC * (A['H1'] @ Wa['DW2'].T) + prop
+    bnd = NET_ACC * (A['H1'] @ Wa['DW2'].T + ba('DB2')) + prop
     p_o = _flip(o, bnd) + prop
+    p_sigma = bnd[:, 0] if vanilla else p_o[:, 0]
     sh = A['sh32'].double()
     p_in = torch.cat([p_o, fb._ulp16(sh) * (fb._mid_dist(sh) <= fb.SH_ABS)], 1)
     act_in, ties = A['CI'].abs(), [tie_h1]
-    for key, wk, act in (('g1', 'CW1', 'G1'), ('g2', 'CW2', 'G2')):
+    for key, wk, bk, act in (('g1', 'CW1', 'CB1', 'G1'), ('g2', 'CW2', 'CB2', 'G2')):
         pre = A['pre'][key]
         prop = p_in @ Wa[wk].T
-        bnd = NET_ACC * (act_in @ Wa[wk].T) + prop
+        bnd = NET_ACC * (act_in @ Wa[wk].T + ba(bk)) + prop
         tie = (pre.abs() <= bnd) & (bnd > 0)
         p_in = torch.where((A[act] > 0) | tie, _flip(pre, bnd) + prop, torch.zeros_like(pre)) + torch.where(tie, pre.abs() + bnd, torch.zeros_like(pre))
         act_in = A[act]
         ties.append(tie)
-    raw = A['G2'] @ W['CW3'].double()[:3].T
+    raw = A['raw'].double()
     prop = p_in @ Wa['CW3'][:3].T
-    bnd = NET_ACC * (A['G2'] @ Wa['CW3'][:3].T) + prop
-    p_raw = _flip(raw, bnd) + prop
+    bnd = NET_ACC * (A['G2'] @ Wa['CW3'][:3].T + (Wa['CB3'][:3] if vanilla else 0.0)) + prop
+    p_raw = bnd if vanilla else _flip(raw, bnd) + prop
     # fp32: the bias add (one rounding of x), expf (<= 2 ulp), 1 / (1 + expf(-raw)) (<= 4 ulp of a value < 1)
-    M_sigma = sigma * (torch.expm1(p_o[:, 0] + EPS32 * x.abs()) + 4 * EPS32)
+    M_sigma = sigma * (torch.expm1(p_sigma + EPS32 * x.abs()) + 4 * EPS32)
     M_rgb = 0.25 * p_raw + 8 * EPS32
     # rows counted as ties: field_bwd_ref's rule (the perturbations above are wider: they also carry upstream flips along)
     tie_rows = torch.stack([t.any(1) for t in fb._tie_masks(A, W)]).any(0)
-    return dict(sigma=sigma, rgb=rgb, M_sigma=M_sigma, M_rgb=M_rgb, tie_rows=tie_rows, out0=A['O'][:, 0])
+    return dict(sigma=sigma, rgb=rgb, M_sigma=M_sigma, M_rgb=M_rgb, tie_rows=tie_rows, out0=out0)
 
 
 def assert_few_ties(tie_rows, what=''):

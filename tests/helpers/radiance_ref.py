@@ -115,10 +115,10 @@ def backward(W, A, masks, dc3, ls, n_feat, n_extra, dtype, store=None, inject=0.
     dG2 = st((D3 @ Wd['W3'][:3]) * m2 + inject * m2)
     dG1 = st((dG2 @ Wd['W2']) * m1 + inject * m1)
     dX = dG1 @ Wd['W1']
-    gW3 = torch.zeros(16, 64, dtype=dtype)
+    gW3 = torch.zeros(16, 64, dtype=dtype, device=D3.device)
     gW3[:3] = D3.T @ A['H2'].to(dtype)
     gp = torch.cat([(dG1.T @ A['X'].to(dtype)).flatten(), (dG2.T @ A['H1'].to(dtype)).flatten(), gW3.flatten()]) / ls
-    gb = torch.zeros(N_BIAS, dtype=dtype)
+    gb = torch.zeros(N_BIAS, dtype=dtype, device=D3.device)
     gb[:64], gb[64:128], gb[128:131] = dG1.sum(0), dG2.sum(0), D3.sum(0)
     ec = n_feat + 16 if extra_col is None else extra_col
     scaled_max = max(float(t.abs().max()) if n else 0.0 for t in (D3, dG2, dG1))
@@ -252,7 +252,7 @@ def check_fwd(got, F, what='rgb'):
 
 # the backward's outputs and the slice of the kernel buffer each is checked on; the last layer's weight and bias gradients come from
 # one fp16 rounding (T_D3) and the fp32 sigmoid', so they are held to RTOL_OUT, two fp16 roundings
-RTOL_OUT = 2.0 ** -10
+RTOL_OUT = fb.RTOL_OUT
 BWD_PARTS = {'W12': ('params', slice(0, 6144), RTOL), 'W3': ('params', slice(6144, N_PARAMS), RTOL_OUT),
              'b12': ('bias', slice(0, 128), RTOL), 'b3': ('bias', slice(128, N_BIAS), RTOL_OUT),
              'd_feat': ('d_feat', slice(None), RTOL), 'd_extra': ('d_extra', slice(None), RTOL)}
