@@ -467,6 +467,18 @@ int nsr_neus_render_rays_fd(const nsr_grid_t* g, const float* rays, const uint32
                             const float* fd_state, const nsr_radiance_t* rp, int32_t vanilla, const void* rgb_params_h, const float* rgb_bias,
                             const float* inv_s, const float* cos_anneal, float* opacity, float* depth, float* comp_rgb, float* comp_normal,
                             uint32_t* ticket, int64_t n_rays, void* stream);
+/* nsr_neus_vertex_rgb: the per-vertex colour of NeuSModel.export (models/neus.py:321-329, export_vertex_color) in ONE kernel: per vertex
+ * of verts f32 [n,3] (world coordinates, device), the SDF field with its analytic normal (weights as nsr_neus_field_fwd_levels, n_active:
+ * device float, 16 for a plain HashGrid), nrm = F.normalize(grad) = g / max(||g||, 1e-12) in fp32, the colour network on
+ * [feature (13) | SH4(-nrm) | nrm] (rp: n_feat 13, n_extra 3; vanilla 0: FullyFused as nsr_radiance_fwd, 1: VanillaMLP as
+ * nsr_radiance_vanilla_fwd with rgb_bias) and rp's colour activation.  Writes rgb f32 [n,3] and nothing else; n = 0 launches nothing.
+ * nsr_neus_vertex_rgb_fd: the same with the finite-difference field of nsr_neus_render_rays_fd (fd_state: device {eps, eps^2, n_active}). */
+int nsr_neus_vertex_rgb(const nsr_grid_t* g, const float* verts, const void* table_h, const float* W1, const float* b1, const float* W2,
+                        const float* b2, float radius, int32_t n_out, const float* n_active, const nsr_radiance_t* rp, int32_t vanilla,
+                        const void* rgb_params_h, const float* rgb_bias, float* rgb, int64_t n, void* stream);
+int nsr_neus_vertex_rgb_fd(const nsr_grid_t* g, const float* verts, const void* table_h, const float* W1, const float* b1, const float* W2,
+                           const float* b2, float radius, int32_t n_out, const float* fd_state, const nsr_radiance_t* rp, int32_t vanilla,
+                           const void* rgb_params_h, const float* rgb_bias, float* rgb, int64_t n, void* stream);
 /* VolumeRadiance (see nsr_radiance_t): feat f32 [n,n_feat], dirs f32 [n,3] (unit view directions, per sample), extra f32 [n,n_extra] (or NULL), params fp16 [7168] in tcnn order,
  * rgb f32 [n,3].  Backward: d_rgb [n,3] -> d_feat, d_extra (either may be NULL), grad_params f32 [7168] (+=);
  * loss_scale <= 0: choose the fp16 dgrad scale from *amax (device float: max |d_rgb|). */

@@ -112,6 +112,8 @@ _SIGNATURES = {
     'nsr_neus_composite_bwd': [P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, I64, P],
     'nsr_neus_render_rays': [P, P, P, I32, P, P, P, P, F32, P, P, P, P, P, F32, I32, P, P, I32, P, P, P, P, P, P, P, P, P, I64, P],
     'nsr_neus_render_rays_fd': [P, P, P, I32, P, P, P, P, F32, P, P, P, P, P, F32, I32, P, P, I32, P, P, P, P, P, P, P, P, P, I64, P],
+    'nsr_neus_vertex_rgb': [P, P, P, P, P, P, P, F32, I32, P, P, I32, P, P, P, I64, P],
+    'nsr_neus_vertex_rgb_fd': [P, P, P, P, P, P, P, F32, I32, P, P, I32, P, P, P, I64, P],
     'nsr_radiance_fwd': [P, P, P, P, P, P, I64, P, P],
     'nsr_radiance_bwd': [P, P, P, P, P, P, F32, P, P, P, P, I64, P, P],
     'nsr_radiance_vanilla_fwd': [P, P, P, P, P, P, P, I64, P, P],

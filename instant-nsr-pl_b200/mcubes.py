@@ -164,12 +164,15 @@ def forward_level_planes(forward_level, chunk):
 
 
 @torch.no_grad()
-def isosurface_slabs(level_planes, radius, resolution, threshold, slab, device):
+def isosurface_slabs(level_planes, radius, resolution, threshold, slab, device, on_slab=None):
     """isosurface() streamed slab by slab: the same two passes, lattice points and mesh (vertex and face order included) for a field
     that gives the same level values.  level_planes(axes, a, b, out) writes the level of the lattice planes [a, b) into out
     [b - a, R, R] (axes: lattice_axes of the pass; forward_level_planes, or a geometry's lattice kernel).  The coarse pass keeps only
     its bounding box; the refined pass's slabs go to the host as they are made, so device memory holds one slab's level planes,
-    vertex map and mesh piece.  -> {'v_pos' [V,3], 't_pos_idx' [F,3]} on the CPU."""
+    vertex map and mesh piece.  -> {'v_pos' [V,3], 't_pos_idx' [F,3]} on the CPU.
+    on_slab(verts) (optional): called with each refined slab's device vertices f32 [V_s,3], in slab order, before they are copied to the
+    host; it returns a dict of per-vertex tensors [V_s, ...], which are concatenated like v_pos and added to the result under their keys
+    (the vertex colour of an export, computed while the slab is still on the device)."""
     r = int(resolution)
 
     def one_pass(vmin, vmax):
@@ -185,5 +188,12 @@ def isosurface_slabs(level_planes, radius, resolution, threshold, slab, device):
     if lo is None:
         return {'v_pos': torch.empty(0, 3), 't_pos_idx': torch.empty(0, 3, dtype=torch.int64)}
     lo_, hi_ = (lo - (hi - lo) * 0.1).clamp(-rad, rad), (hi + (hi - lo) * 0.1).clamp(-rad, rad)
-    pieces = [(v.cpu(), f.cpu()) for v, f in one_pass(lo_.tolist(), hi_.tolist())]
-    return {'v_pos': torch.cat([v for v, _ in pieces]), 't_pos_idx': torch.cat([f for _, f in pieces])}
+    pieces, extra = [], []
+    for v, f in one_pass(lo_.tolist(), hi_.tolist()):
+        if on_slab is not None:
+            extra.append({k: t.cpu() for k, t in on_slab(v).items()})
+        pieces.append((v.cpu(), f.cpu()))
+    mesh = {'v_pos': torch.cat([v for v, _ in pieces]), 't_pos_idx': torch.cat([f for _, f in pieces])}
+    if extra:
+        mesh.update({k: torch.cat([e[k] for e in extra]) for k in extra[0]})
+    return mesh

@@ -50,10 +50,11 @@ class BaseImplicitGeometry(BaseModel):
         return mcubes.forward_level_planes(self.forward_level, chunk)
 
     @torch.no_grad()
-    def isosurface(self):
+    def isosurface(self, on_slab=None):
         """models/geometry.py:80-112: coarse + refined marching cubes over the level field, here extracted on the GPU (nsr_b200.mcubes).
         With ``isosurface.fused: true`` both passes stream over slabs of ``isosurface.slab`` x-planes (default 64), the level of a fused
-        SDF geometry coming from its lattice kernel (fused_level_unsupported() says why another geometry uses forward_level)."""
+        SDF geometry coming from its lattice kernel (fused_level_unsupported() says why another geometry uses forward_level).
+        on_slab: mcubes.isosurface_slabs's per-slab callback (only with isosurface.fused)."""
         iso = self.config.get('isosurface', None)
         if iso is None:
             raise NotImplementedError
@@ -61,7 +62,9 @@ class BaseImplicitGeometry(BaseModel):
         device = next(self.parameters()).device
         if iso.get('fused', False):
             return mcubes.isosurface_slabs(self._level_planes(iso.chunk), self.radius, iso.resolution, iso.threshold, iso.get('slab', 64),
-                                           device)
+                                           device, on_slab=on_slab)
+        if on_slab is not None:
+            raise ValueError('isosurface: a per-slab callback needs the slab-streamed extraction (isosurface.fused: true)')
         return mcubes.isosurface(self.forward_level, self.radius, iso.resolution, iso.threshold, iso.chunk, device)
 
 

@@ -172,6 +172,13 @@ class NeRFModel(BaseModel):
         losses.update(self.texture.regularizations(out))
         return losses
 
+    def fused_export_unsupported(self, export_config):
+        """why export() keeps the per-op colour pass under ``fused_vertex_color: true`` (the per-vertex colour kernel serves the NeuS
+        fields only), mirroring NeuSModel.fused_export_unsupported"""
+        if not export_config.get('fused_vertex_color', False):
+            return 'fused_vertex_color is off'
+        return 'the per-vertex colour kernel serves the NeuS SDF fields: a NeRF density field keeps the per-op colour pass'
+
     @torch.no_grad()
     def export(self, export_config):
         """models/nerf.py:153-161: isosurface mesh (+ per-vertex colour seen from above)"""

@@ -366,23 +366,11 @@ class NeuSModel(BaseModel):
         e = lambda k: torch.empty(0, k, device=dev)
         return self.texture._fused_spec(e(n_feat), e(3), (e(3),))
 
-    @torch.no_grad()
-    def _render_fused(self, rays):
-        """eval-mode forward() on the per-ray kernel: passes of config.render_chunk rays, outputs kept on the device and copied to
-        the CPU once; the learned background runs its sync-free executor (NerfBackgroundFused.render(static=True)) per pass."""
-        import math
-        cfg, geo, tex = self.config, self.geometry, self.texture
-        rays = rays.float().contiguous()
-        dev = rays.device
+    def _fused_field_args(self, dev):
+        """the arguments the per-ray renderer and the per-vertex colour kernel share: dict(grid_spec, radius, table_h, W1, b1, W2, b2,
+        n_active, rspec, rgb_params_h, rgb_bias, fd_state) (finite-difference normals: raises until update_step has set eps)"""
+        geo, tex = self.geometry, self.texture
         spec = self._render_spec(dev)
-        grid = self.occupancy_grid
-        if self._march_static is None:
-            r = float(cfg.radius)
-            self._march_static = (ops.march_struct(grid.roi_host(), grid._res, ContractionType.AABB.value, self.render_step_size, 0.0),
-                                  int(math.ceil(2.0 * math.sqrt(3.0) * r / self.render_step_size)) + 2)
-        ms, cap_per_ray = self._march_static
-        if self._cos_dev is None or self._cos_dev.device != dev:
-            self._cos_dev = torch.full((1,), float(self.cos_anneal_ratio), device=dev)
         enc = geo._fd_grid()
         W1, b1, W2, b2 = geo._effective_weights()
         fd_state = None
@@ -391,19 +379,40 @@ class NeuSModel(BaseModel):
             fd_state, n_active = geo._fd_state, None
         else:
             n_active = geo._fd_state[2:] if geo._progressive else torch.full((1,), 16.0, device=dev)
-        inv_s = self.variance.inv_s.clip(1e-6, 1e6).reshape(1)
         if spec.vanilla:
             weights, rgb_bias = ops.pack_vanilla_radiance(tex.network.linear_params())
             rgb_params = weights.to(torch.float16)
         else:
             rgb_params, rgb_bias = tex.network._params_half(), None
+        return dict(grid_spec=enc.grid, radius=geo.radius, table_h=enc._params_half(), W1=W1, b1=b1, W2=W2, b2=b2, n_active=n_active,
+                    rspec=spec, rgb_params_h=rgb_params, rgb_bias=rgb_bias, fd_state=fd_state)
+
+    @torch.no_grad()
+    def _render_fused(self, rays):
+        """eval-mode forward() on the per-ray kernel: passes of config.render_chunk rays, outputs kept on the device and copied to
+        the CPU once; the learned background runs its sync-free executor (NerfBackgroundFused.render(static=True)) per pass."""
+        import math
+        cfg = self.config
+        rays = rays.float().contiguous()
+        dev = rays.device
+        grid = self.occupancy_grid
+        if self._march_static is None:
+            r = float(cfg.radius)
+            self._march_static = (ops.march_struct(grid.roi_host(), grid._res, ContractionType.AABB.value, self.render_step_size, 0.0),
+                                  int(math.ceil(2.0 * math.sqrt(3.0) * r / self.render_step_size)) + 2)
+        ms, cap_per_ray = self._march_static
+        if self._cos_dev is None or self._cos_dev.device != dev:
+            self._cos_dev = torch.full((1,), float(self.cos_anneal_ratio), device=dev)
+        fa = self._fused_field_args(dev)
+        inv_s = self.variance.inv_s.clip(1e-6, 1e6).reshape(1)
         bg_fused = self._static_background() if cfg.learned_background else None
         chunk = int(cfg.get('render_chunk', 65536))
         fg, bg, overflow = [], [], []
         for s in range(0, rays.shape[0], chunk):
             r = rays[s:s + chunk]
-            fg.append(ops.neus_render_rays(ms, r, grid.bits(), grid.coarse_bits(), cap_per_ray, enc.grid, geo.radius, enc._params_half(), W1, b1,
-                                           W2, b2, n_active, spec, rgb_params, rgb_bias, inv_s, self._cos_dev, fd_state=fd_state))
+            fg.append(ops.neus_render_rays(ms, r, grid.bits(), grid.coarse_bits(), cap_per_ray, fa['grid_spec'], fa['radius'], fa['table_h'],
+                                           fa['W1'], fa['b1'], fa['W2'], fa['b2'], fa['n_active'], fa['rspec'], fa['rgb_params_h'],
+                                           fa['rgb_bias'], inv_s, self._cos_dev, fd_state=fa['fd_state']))
             if bg_fused is not None:
                 o = bg_fused.render(r, None, static=True)
                 off = bg_fused.last_offsets_k
@@ -438,9 +447,51 @@ class NeuSModel(BaseModel):
         losses.update(self.texture.regularizations(out))
         return losses
 
+    def fused_export_unsupported(self, export_config):
+        """None when export() colours the vertices with the per-vertex kernel (ops.neus_vertex_rgb; export key
+        ``fused_vertex_color: true``), else why it keeps the per-op colour pass (a message)."""
+        if not export_config.get('fused_vertex_color', False):
+            return 'fused_vertex_color is off'
+        geo = self.geometry
+        if not geo.config.get('fused', True):
+            return 'the geometry runs the per-op path (fused: false)'
+        if not (geo._fused or geo._fused_fd):
+            if geo._progressive and geo.grad_type == 'analytic' and not geo.config.get('fused_progressive', False):
+                return 'a ProgressiveBandHashGrid runs the fused field only with fused_progressive: true'
+            return ('the geometry is not a fused SDF field shape (include_xyz HashGrid or ProgressiveBandHashGrid L=16 F=2 + sphere-init '
+                    'VanillaMLP 35 -> 64 -> n_out)')
+        if geo.n_output_dims != 13:
+            return f'the colour input is [feature 13 | SH4 | normal]: feature_dim is {geo.n_output_dims}'
+        if self._render_spec(next(self.parameters()).device) is None:
+            return ('the colour network is not a fused shape (CUDA, SH4 directions + FullyFusedMLP or ReLU VanillaMLP 64 x 2 with the '
+                    'activations VolumeRadiance fuses)')
+        return None
+
+    @torch.no_grad()
+    def _export_fused(self, export_config):
+        """export() with the per-vertex colour kernel: inside the slab loop under isosurface.fused (the vertices are coloured on the
+        device before their copy to the host), else over the finished mesh in chunk_size slices"""
+        dev = next(self.parameters()).device
+        fa = self._fused_field_args(dev)
+
+        def colour(v):
+            return ops.neus_vertex_rgb(verts=v, **fa)
+
+        if self.geometry.config.isosurface.get('fused', False):
+            mesh = self.geometry.isosurface(on_slab=lambda v: {'v_rgb': colour(v)})
+            mesh.setdefault('v_rgb', torch.zeros(0, 3))
+            return mesh
+        mesh = self.isosurface()
+        v, chunk = mesh['v_pos'], int(export_config.chunk_size)
+        mesh['v_rgb'] = torch.cat([torch.zeros(0, 3)] + [colour(v[s:s + chunk].to(dev)).cpu() for s in range(0, v.shape[0], chunk)])
+        return mesh
+
     @torch.no_grad()
     def export(self, export_config):
-        """models/neus.py:321-329: isosurface mesh (+ per-vertex "albedo": colour seen along the normal)"""
+        """models/neus.py:321-329: isosurface mesh (+ per-vertex "albedo": colour seen along the normal).  With the export key
+        ``fused_vertex_color: true`` the colour comes from one per-vertex kernel (fused_export_unsupported() says when it cannot)."""
+        if export_config.export_vertex_color and self.fused_export_unsupported(export_config) is None:
+            return self._export_fused(export_config)
         mesh = self.isosurface()
         if export_config.export_vertex_color and mesh['v_pos'].shape[0] == 0:
             mesh['v_rgb'] = torch.zeros(0, 3)        # nothing crossed the threshold (the reference would fail on the empty chunk list)

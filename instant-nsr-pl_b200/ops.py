@@ -929,6 +929,26 @@ def neus_render_rays(ms, rays, bits, coarse_bits, cap_per_ray, grid_spec, radius
     return {'opacity': opacity, 'depth': depth, 'comp_rgb': comp_rgb, 'comp_normal': comp_normal, 'counts': counts}
 
 
+def neus_vertex_rgb(grid_spec, radius, verts, table_h, W1, b1, W2, b2, n_active, rspec, rgb_params_h, rgb_bias, fd_state=None):
+    """per-vertex colour of a NeuS mesh export (models/neus.py:321-329): the SDF field's feature and normal n = F.normalize(grad) at each
+    vertex, then the colour network on [feature | SH4(-n) | n] with rspec's activation, in one kernel (nsr_neus_vertex_rgb).  verts: CUDA
+    f32 [n,3] in world coordinates.  The other arguments are neus_render_rays's (n_active: the analytic field's active levels, or
+    fd_state for the finite-difference field, nsr_neus_vertex_rgb_fd).  No autograd.  -> rgb f32 [n,3]."""
+    field_state = n_active if fd_state is None else fd_state
+    check_cuda(verts, table_h, W1, W2, field_state, rgb_params_h, what='neus_vertex_rgb')
+    if verts.dim() != 2 or verts.shape[-1] != 3:
+        raise ValueError(f'neus_vertex_rgb: verts must be [n, 3], got {tuple(verts.shape)}')
+    verts = contig(verts.detach(), torch.float32)
+    n = verts.shape[0]
+    rgb = torch.empty(n, 3, device=verts.device)
+    if n > 0:
+        f32 = lambda t: contig(t.detach(), torch.float32)
+        lib.call('nsr_neus_vertex_rgb' if fd_state is None else 'nsr_neus_vertex_rgb_fd', grid_spec.ref(), ptr(verts), ptr(table_h),
+                 ptr(f32(W1)), ptr(f32(b1)), ptr(f32(W2)), ptr(f32(b2)), float(radius), int(W2.shape[0]), ptr(f32(field_state)),
+                 rspec.ref(), int(rspec.vanilla), ptr(rgb_params_h), ptr(None if rgb_bias is None else f32(rgb_bias)), ptr(rgb), n, stream())
+    return rgb
+
+
 def nerf_render_rays(f, ms, rays, bits, coarse_bits, bound, dparams_h, cparams_h, early_stop_eps, near=0.0, far=1e10):
     """NeRF eval render of a pass of rays (NeRFModel.forward_ in eval mode, models/nerf.py:82-109): marcher -> one kernel per ray warp
     (nsr_nerf_render_rays).  f: the field's NerfT; ms: march_struct with the same contraction.  AABB (0): nsr_march_rays_alloc over bits /
