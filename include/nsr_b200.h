@@ -479,6 +479,19 @@ int nsr_neus_vertex_rgb(const nsr_grid_t* g, const float* verts, const void* tab
 int nsr_neus_vertex_rgb_fd(const nsr_grid_t* g, const float* verts, const void* table_h, const float* W1, const float* b1, const float* W2,
                            const float* b2, float radius, int32_t n_out, const float* fd_state, const nsr_radiance_t* rp, int32_t vanilla,
                            const void* rgb_params_h, const float* rgb_bias, float* rgb, int64_t n, void* stream);
+/* Mesh export of the fused NeRF density field (NeRFModel.export, models/nerf.py:153-161); f: the field (16-level F=2 grid, radius,
+ * density_bias, contraction 0 AABB or 2 UN_BOUNDED_SPHERE), dparams_h: fp16 [density network 3072 | table] as nsr_nerf_density reads it.
+ * The contraction follows contract_to_unisphere as torch computes it: (x + r) * (1 / (2r)), and for the sphere |v|^2 = (x^2 + z^2) + y^2.
+ * nsr_nerf_density_lattice: VolumeDensity.forward_level on the planes [ix0, ix0 + n_planes) of the lattice ax f32 [nx] x ay [ny] x az [nz]
+ *   (world coordinates, device) into level f32 [n_planes, ny, nz] ('ij' order, z fastest): -exp(fp16(raw0 + density_bias)), raw0 the fp16
+ *   network output -- the bias is added to the fp16 output and rounded, as forward_level does.  Writes nothing but the level.
+ * nsr_nerf_vertex_rgb: the export's vertex colour per vertex of verts f32 [n,3] (world coordinates, device): the density network's 16
+ *   outputs as the feature, the colour network (cparams_h fp16 [7168]; rp: n_feat 16, n_extra 0) on [feature | SH4(0,0,-1)] with rp's
+ *   activation as nsr_radiance_fwd, clamped to [0,1].  Writes rgb f32 [n,3] and nothing else; n = 0 launches nothing. */
+int nsr_nerf_density_lattice(const nsr_nerf_t* f, const float* ax, const float* ay, const float* az, int32_t nx, int32_t ny, int32_t nz,
+                             int32_t ix0, int32_t n_planes, const void* dparams_h, float* level, void* stream);
+int nsr_nerf_vertex_rgb(const nsr_nerf_t* f, const float* verts, const void* dparams_h, const nsr_radiance_t* rp, const void* cparams_h,
+                        float* rgb, int64_t n, void* stream);
 /* VolumeRadiance (see nsr_radiance_t): feat f32 [n,n_feat], dirs f32 [n,3] (unit view directions, per sample), extra f32 [n,n_extra] (or NULL), params fp16 [7168] in tcnn order,
  * rgb f32 [n,3].  Backward: d_rgb [n,3] -> d_feat, d_extra (either may be NULL), grad_params f32 [7168] (+=);
  * loss_scale <= 0: choose the fp16 dgrad scale from *amax (device float: max |d_rgb|). */

@@ -216,6 +216,71 @@ class _NerfRenderRays(torch.autograd.Function):
         return gd, gc, None, None, None
 
 
+def nerf_field_struct(grid, radius, density_bias, contraction_type):
+    """nsr_nerf_t (NerfT) of a fused NeRF density field: its GridSpec, radius, density_bias and contraction (nerfacc.ContractionType)"""
+    s = NerfT()
+    s.grid = grid.struct
+    s.radius = float(radius)
+    s.density_bias = float(density_bias)
+    s.feature_dim, s.density_hidden, s.color_hidden = 16, 1, 2
+    s.contraction = contraction_type.value
+    return s
+
+
+def density_field_unsupported(geo):
+    """None when the geometry is the density field the fused NeRF kernels implement (volume-density: HashGrid L=16 F=2 -> FullyFusedMLP
+    32 -> 64 (ReLU) -> 16 linear outputs, trunc_exp density, no feature activation), else what it lacks (a message)"""
+    from . import tcnn
+    from .models.fields import VolumeDensity
+    try:
+        if not isinstance(geo, VolumeDensity):
+            return f'the geometry is a {type(geo).__name__}, not a volume-density field'
+        net = geo.encoding_with_network
+        if not isinstance(net, tcnn.NetworkWithInputEncoding):
+            return ('the density field is not HashGrid + FullyFusedMLP (tcnn NetworkWithInputEncoding): a VanillaFrequency + VanillaMLP '
+                    'field (nerf_vanilla) has no fused kernel')
+        if net.grid.n_levels != 16 or net.mlp.n_hidden != 1:
+            return 'the density network is not HashGrid L=16 F=2 -> FullyFusedMLP 32 -> 64 -> out (one hidden layer)'
+        if geo.n_output_dims != 16:
+            return f'the density network emits [density | feature] 16 wide: feature_dim is {geo.n_output_dims}'
+        if geo.config.get('density_activation') != 'trunc_exp':
+            return f'the density activation is trunc_exp: density_activation is {geo.config.get("density_activation")!r}'
+        if 'feature_activation' in geo.config:
+            return f'the feature is the raw network output: feature_activation is {geo.config.feature_activation!r}'
+        if net.mlp.struct.activation != 1 or net.mlp.struct.out_activation != 0:
+            return 'the density network has ReLU hidden layers and a linear output'
+    except AttributeError:
+        return 'the density field is not the fused shape'
+    return None
+
+
+def color_network_unsupported(tex):
+    """None when the texture is the colour network the fused NeRF kernels implement (volume-radiance: [feature 16 | SH4(dir)] ->
+    FullyFusedMLP 32 -> 64 -> 64 (ReLU) -> 3 with one sigmoid, as the network's output activation or as color_activation), else what it
+    lacks (a message)"""
+    from . import tcnn
+    from .models.fields import VolumeRadiance
+    try:
+        if not isinstance(tex, VolumeRadiance):
+            return f'the texture is a {type(tex).__name__}, not a volume-radiance field'
+        net = tex.network
+        if not (isinstance(net, tcnn.Network) and net.mlp.n_hidden == 2 and net.mlp.n_in == 32):
+            return 'the colour network is not FullyFusedMLP 32 -> 64 -> 64 -> 3'
+        if not (isinstance(tex.encoding.encoding, tcnn.Encoding) and tex.encoding.encoding.otype == 'SphericalHarmonics'
+                and not tex.encoding.include_xyz and tex.config.input_feature_dim == 16):
+            return 'the colour input is not [feature 16 | SH4(dir)]'
+        if net.mlp.struct.activation != 1:
+            return 'the colour network has ReLU hidden layers'
+        net_act = str(net.network_config.get('output_activation', 'None')).lower()
+        col_act = str(tex.config.get('color_activation', 'none')).lower()
+        if sorted([net_act, col_act]) != ['none', 'sigmoid']:
+            return (f'the colour takes one sigmoid, as the network output activation or as color_activation: got output_activation '
+                    f'{net_act!r}, color_activation {col_act!r}')
+    except AttributeError:
+        return 'the colour network is not the fused shape'
+    return None
+
+
 class NerfFused:
     """Fused executor attached to a NeRFModel whose config has the nerf-blender shape: the AABB scene of nerf-blender, or (config key
     ``fused_unbounded``) the unbounded scene of nerf-colmap -- UN_BOUNDED_SPHERE contraction, cone marching from the near to the far
@@ -229,14 +294,8 @@ class NerfFused:
         self.grid = self.net.grid
         self.n_dparams, self.n_cparams = self.net.params.numel(), self.cnet.params.numel()
         r = float(model.config.radius)
-        s = NerfT()
-        s.grid = self.grid.struct
-        s.radius = r
-        s.density_bias = float(geo.config.density_bias)
-        s.feature_dim, s.density_hidden, s.color_hidden = 16, 1, 2
         self.contracted = model.contraction_type == ContractionType.UN_BOUNDED_SPHERE
-        s.contraction = model.contraction_type.value
-        self.struct = s
+        self.struct = nerf_field_struct(self.grid, r, geo.config.density_bias, model.contraction_type)
         self.march = ops.march_struct([-r, -r, -r, r, r, r], model.occupancy_grid_res, model.contraction_type.value, model.render_step_size,
                                       model.cone_angle)
         if self.contracted:
@@ -278,26 +337,11 @@ class NerfFused:
     @staticmethod
     def try_build(model):
         """Return a NerfFused if the model is exactly the shape the fused kernels implement, else None."""
-        from . import tcnn
-        from .models.fields import VolumeDensity, VolumeRadiance
         cfg = model.config
-        geo, tex = model.geometry, model.texture
         try:
             # learned_background (nerf-colmap: contracted, cone-marched) is opt-in through the model config key fused_unbounded
-            ok = ((not cfg.learned_background or cfg.get('fused_unbounded', False)) and cfg.grid_prune and isinstance(geo, VolumeDensity) and isinstance(tex, VolumeRadiance)
-                  and isinstance(geo.encoding_with_network, tcnn.NetworkWithInputEncoding)
-                  and geo.encoding_with_network.grid.n_levels == 16 and geo.encoding_with_network.mlp.n_hidden == 1
-                  and geo.n_output_dims == 16 and geo.config.get('density_activation') == 'trunc_exp'
-                  and 'feature_activation' not in geo.config
-                  and isinstance(tex.network, tcnn.Network) and tex.network.mlp.n_hidden == 2 and tex.network.mlp.n_in == 32
-                  and isinstance(tex.encoding.encoding, tcnn.Encoding) and tex.encoding.encoding.otype == 'SphericalHarmonics'
-                  and not tex.encoding.include_xyz and tex.config.input_feature_dim == 16)
-            # the kernels hard-code ReLU hidden layers and a linear density output: anything else runs on the composed path
-            dm, cm = geo.encoding_with_network.mlp.struct, tex.network.mlp.struct
-            ok = ok and dm.activation == 1 and dm.out_activation == 0 and cm.activation == 1
-            net_act = str(tex.network.network_config.get('output_activation', 'None')).lower()
-            col_act = str(tex.config.get('color_activation', 'none')).lower()
-            ok = ok and sorted([net_act, col_act]) == ['none', 'sigmoid']
+            ok = ((not cfg.learned_background or cfg.get('fused_unbounded', False)) and cfg.grid_prune
+                  and density_field_unsupported(model.geometry) is None and color_network_unsupported(model.texture) is None)
         except AttributeError:
             ok = False
         return NerfFused(model) if ok else None

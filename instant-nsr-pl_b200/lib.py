@@ -137,6 +137,8 @@ _SIGNATURES = {
     'nsr_mc_count_slab': [P, I32, I32, I32, I32, I32, F32, I32, P, P, P],
     'nsr_mc_emit_slab': [P, I32, I32, I32, I32, I32, F32, I32, P, P, P, P, P, I64, P, I64, I64, P],
     'nsr_nerf_density': [P, P, P, P, I64, P],
+    'nsr_nerf_density_lattice': [P, P, P, P, I32, I32, I32, I32, I32, P, P, P],
+    'nsr_nerf_vertex_rgb': [P, P, P, P, P, P, I64, P],
     'nsr_nerf_prepass': [P, P, P, P, P, P, P, I64, P, P],
     'nsr_compact_prefix': [P, P, P, P, P, P, P, P, P, P, I64, P],
     'nsr_nerf_render_fwd': [P, P, P, P, P, P, P, P, P, P, P, P, P, P, P, I64, P, P],

@@ -96,6 +96,47 @@ class VolumeDensity(BaseImplicitGeometry):
     def forward_level(self, points):
         return -self._density(self._raw(points)[..., 0])
 
+    def fused_export_field_unsupported(self):
+        """None when the export kernels (ops.nerf_density_lattice / ops.nerf_vertex_rgb; geometry key ``fused_export: true``) can run this
+        density field, else why not (a message)"""
+        from ..fused import density_field_unsupported
+        if not self.config.get('fused_export', False):
+            return 'fused_export is off'
+        why = density_field_unsupported(self)
+        if why is not None:
+            return why
+        if self.encoding_with_network.mlp.backend != 'mma_sync':
+            return (f'the density network runs on the {self.encoding_with_network.mlp.backend} backend: the export kernels run the '
+                    'mma_sync chain of its default backend')
+        if self.contraction_type not in (ContractionType.AABB, ContractionType.UN_BOUNDED_SPHERE):
+            return f'the export kernels contract world points by AABB or UN_BOUNDED_SPHERE, the field uses {self.contraction_type}'
+        return None
+
+    def fused_level_unsupported(self):
+        """None when isosurface.fused evaluates the level with the lattice kernel (ops.nerf_density_lattice; geometry key
+        ``fused_export: true`` on the fused density field shape), else why the level streams through forward_level (a message)."""
+        why = self.fused_export_field_unsupported()
+        if why is None:
+            return None
+        if why == 'fused_export is off':
+            return 'VolumeDensity evaluates its level with the lattice kernel only under fused_export: true: its level streams through forward_level'
+        return f'{why}: the VolumeDensity level streams through forward_level'
+
+    def _nerf_struct(self):
+        """nsr_nerf_t of this field for the export kernels"""
+        from ..fused import nerf_field_struct
+        return nerf_field_struct(self.encoding_with_network.grid, self.radius, self.config.density_bias, self.contraction_type)
+
+    def _level_planes(self, chunk):
+        if self.fused_level_unsupported() is not None:
+            return super()._level_planes(chunk)
+        f = self._nerf_struct()
+        dparams_h = self.encoding_with_network._params_half()
+
+        def planes(axes, a, b, out):
+            ops.nerf_density_lattice(f, axes, a, b, dparams_h, out)
+        return planes
+
     def update_step(self, epoch, global_step):
         update_module_step(self.encoding_with_network, epoch, global_step)
 

@@ -172,16 +172,68 @@ class NeRFModel(BaseModel):
         losses.update(self.texture.regularizations(out))
         return losses
 
+    def _export_spec(self, dev):
+        """the colour network's RadianceSpec on [feature 16 | SH4(dir)] (VolumeRadiance._fused_spec: None unless CUDA, mma_sync backend)"""
+        e = lambda k: torch.empty(0, k, device=dev)
+        return self.texture._fused_spec(e(16), e(3), ())
+
     def fused_export_unsupported(self, export_config):
-        """why export() keeps the per-op colour pass under ``fused_vertex_color: true`` (the per-vertex colour kernel serves the NeuS
-        fields only), mirroring NeuSModel.fused_export_unsupported"""
+        """None when export() colours the vertices with the per-vertex kernel (ops.nerf_vertex_rgb; export key ``fused_vertex_color: true``
+        and geometry key ``fused_export: true``), else why it keeps the per-op colour pass (a message); mirrors
+        NeuSModel.fused_export_unsupported"""
         if not export_config.get('fused_vertex_color', False):
             return 'fused_vertex_color is off'
-        return 'the per-vertex colour kernel serves the NeuS SDF fields: a NeRF density field keeps the per-op colour pass'
+        geo = self.geometry
+        why = geo.fused_export_field_unsupported()
+        if why == 'fused_export is off':
+            return ('the per-vertex colour kernel serves a NeRF density field only under the geometry key fused_export: true: without it '
+                    'the field keeps the per-op colour pass')
+        if why is not None:
+            return why
+        from ..fused import color_network_unsupported
+        why = color_network_unsupported(self.texture)
+        if why is not None:
+            return why
+        if self.texture.network.mlp.backend != 'mma_sync':
+            return (f'the colour network runs on the {self.texture.network.mlp.backend} backend: the per-vertex kernel runs the mma_sync '
+                    'chain of its default backend')
+        if self._export_spec(next(self.parameters()).device) is None:
+            return ('the colour network is not a fused shape (CUDA, SH4 directions + FullyFusedMLP 32 -> 64 -> 64 -> 3 with the '
+                    'activations VolumeRadiance fuses)')
+        return None
+
+    def _fused_export_args(self, dev):
+        """the arguments of ops.nerf_vertex_rgb besides the vertices: dict(f, dparams_h, rspec, cparams_h)"""
+        geo = self.geometry
+        return dict(f=geo._nerf_struct(), dparams_h=geo.encoding_with_network._params_half(), rspec=self._export_spec(dev),
+                    cparams_h=self.texture.network._params_half())
+
+    @torch.no_grad()
+    def _export_fused(self, export_config):
+        """export() with the per-vertex colour kernel: inside the slab loop under isosurface.fused (the vertices are coloured on the
+        device before their copy to the host), else over the finished mesh in chunk_size slices"""
+        dev = next(self.parameters()).device
+        fa = self._fused_export_args(dev)
+
+        def colour(v):
+            return ops.nerf_vertex_rgb(verts=v, **fa)
+
+        if self.geometry.config.isosurface.get('fused', False):
+            mesh = self.geometry.isosurface(on_slab=lambda v: {'v_rgb': colour(v)})
+            mesh.setdefault('v_rgb', torch.zeros(0, 3))
+            return mesh
+        mesh = self.isosurface()
+        v, chunk = mesh['v_pos'], int(export_config.chunk_size)
+        mesh['v_rgb'] = torch.cat([torch.zeros(0, 3)] + [colour(v[s:s + chunk].to(dev)).cpu() for s in range(0, v.shape[0], chunk)])
+        return mesh
 
     @torch.no_grad()
     def export(self, export_config):
-        """models/nerf.py:153-161: isosurface mesh (+ per-vertex colour seen from above)"""
+        """models/nerf.py:153-161: isosurface mesh (+ per-vertex colour seen from above).  With the export key
+        ``fused_vertex_color: true`` and the geometry key ``fused_export: true`` the colour comes from one per-vertex kernel
+        (fused_export_unsupported() says when it cannot)."""
+        if export_config.export_vertex_color and self.fused_export_unsupported(export_config) is None:
+            return self._export_fused(export_config)
         mesh = self.isosurface()
         if export_config.export_vertex_color and mesh['v_pos'].shape[0] == 0:
             mesh['v_rgb'] = torch.zeros(0, 3)        # nothing crossed the threshold (the reference would fail on the empty chunk list)

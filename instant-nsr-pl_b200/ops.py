@@ -949,6 +949,40 @@ def neus_vertex_rgb(grid_spec, radius, verts, table_h, W1, b1, W2, b2, n_active,
     return rgb
 
 
+def nerf_density_lattice(f, axes, a, b, dparams_h, out):
+    """VolumeDensity.forward_level of the fused NeRF density field f (NerfT: grid, radius, density_bias, contraction) on the x-planes [a, b)
+    of the lattice axes[0] x axes[1] x axes[2] (world coordinates, CUDA fp32 vectors) into out fp32 [b - a, ny, nz] ('ij' order), in one
+    kernel (nsr_nerf_density_lattice).  dparams_h: fp16 [density network | table] (tcnn.NetworkWithInputEncoding._params_half())."""
+    ax, ay, az = (contig(t, torch.float32) for t in axes)
+    check_cuda(ax, ay, az, dparams_h, out, what='nerf_density_lattice')
+    nx, ny, nz = ax.numel(), ay.numel(), az.numel()
+    if out.dtype != torch.float32 or not out.is_contiguous() or tuple(out.shape) != (b - a, ny, nz):
+        raise ValueError(f'nerf_density_lattice: out must be a contiguous float32 [{b - a}, {ny}, {nz}] tensor, got {out.dtype} {tuple(out.shape)}')
+    if b <= a:
+        return out
+    lib.call('nsr_nerf_density_lattice', _C.byref(f), ptr(ax), ptr(ay), ptr(az), nx, ny, nz, int(a), int(b - a), ptr(dparams_h), ptr(out),
+             stream())
+    return out
+
+
+def nerf_vertex_rgb(f, verts, dparams_h, rspec, cparams_h):
+    """the vertex colour of a NeRF mesh export (models/nerf.py:153-161): texture(feature, (0,0,-1)).clamp(0,1) with feature the density
+    network's 16 outputs at each vertex, in one kernel (nsr_nerf_vertex_rgb).  f: NerfT of the field; verts: CUDA f32 [n,3] in world
+    coordinates; rspec: the colour network's RadianceSpec (16 features, no extra input); cparams_h: its fp16 params [7168].  No autograd.
+    -> rgb f32 [n,3]."""
+    check_cuda(verts, dparams_h, cparams_h, what='nerf_vertex_rgb')
+    if verts.dim() != 2 or verts.shape[-1] != 3:
+        raise ValueError(f'nerf_vertex_rgb: verts must be [n, 3], got {tuple(verts.shape)}')
+    if rspec.vanilla or cparams_h.shape[0] != 64 * 32 + 64 * 64 + 16 * 64:
+        raise ValueError('nerf_vertex_rgb: the colour network must be the FullyFused 32 -> 64 -> 64 -> 3 of 7168 parameters')
+    verts = contig(verts.detach(), torch.float32)
+    n = verts.shape[0]
+    rgb = torch.empty(n, 3, device=verts.device)
+    if n > 0:
+        lib.call('nsr_nerf_vertex_rgb', _C.byref(f), ptr(verts), ptr(dparams_h), rspec.ref(), ptr(cparams_h), ptr(rgb), n, stream())
+    return rgb
+
+
 def nerf_render_rays(f, ms, rays, bits, coarse_bits, bound, dparams_h, cparams_h, early_stop_eps, near=0.0, far=1e10):
     """NeRF eval render of a pass of rays (NeRFModel.forward_ in eval mode, models/nerf.py:82-109): marcher -> one kernel per ray warp
     (nsr_nerf_render_rays).  f: the field's NerfT; ms: march_struct with the same contraction.  AABB (0): nsr_march_rays_alloc over bits /

@@ -14,7 +14,18 @@ medians over --runs runs after one warm-up run each.  Prints one JSON line per w
 torch.cuda.max_memory_allocated above what was allocated before the call, vertex and face counts, and the card name and power limit
 read in the same run.
 
+With --nerf it measures the NeRF density fields instead: nerf-blender (AABB) and nerf-colmap (UN_BOUNDED_SPHERE), density shape of
+smoke(), at 256 (the configs' resolution), 512, 1024 and 2048, three ways:
+
+  default       the dense path above (up to 1024: at 2048 its level grid and vertex map alone take 64 GiB);
+  fused         isosurface.fused: true, the level streamed through forward_level (per-op hash grid, network and activation);
+  fused_export  isosurface.fused: true with the geometry key fused_export: true, the level from nsr_nerf_density_lattice.
+
+The three paths alternate run by run (2048: one timed run each, after the 1024 warm-up of the same kernels).  Besides the time and
+peak lines it prints the device bytes each path writes per lattice point, computed from the tensor shapes of its code (not measured).
+
     python tools/isosurface_bench.py [--runs 3] [--only neus-blender] [--no-large]
+    python tools/isosurface_bench.py --nerf [--runs 3] [--only nerf-colmap] [--res 256,512,1024,2048]
 """
 import argparse
 import json
@@ -30,8 +41,8 @@ from nsr_b200 import configs, models, synthetic
 
 
 def build(name, dev, resolution, levels=None):
-    if name == 'nerf-blender':
-        cfg = configs.nerf_blender()
+    if name in ('nerf-blender', 'nerf-colmap'):
+        cfg = configs.nerf_blender() if name == 'nerf-blender' else configs.nerf_colmap()
         torch.manual_seed(0)
         model = models.make('nerf', cfg).to(dev)
         net = model.geometry.encoding_with_network
@@ -77,6 +88,64 @@ def run(model, fused):
     return dt, torch.cuda.max_memory_allocated() - base, mesh
 
 
+NERF_WAYS = ('default', 'fused', 'fused_export')
+DENSE_MAX = 1024
+
+
+def run_nerf(model, way):
+    """isosurface() of a NeRF model on one of NERF_WAYS"""
+    geo = model.geometry
+    geo.config['fused_export'] = way == 'fused_export'
+    dt, peak, mesh = run(model, way != 'default')
+    assert (geo.fused_level_unsupported() is None) == (way == 'fused_export')
+    return dt, peak, mesh
+
+
+def level_bytes_per_point(sphere):
+    """device bytes written per lattice point by each level path, from the shapes and dtypes of the tensors its code makes"""
+    f32, f16, i64, b8 = 4, 2, 8, 1
+    per_op = [('arange', i64), ('a + idx // (ny nz)', 2 * i64), ('(idx // nz) % ny', 2 * i64), ('idx % nz', i64), ('three axis gathers', 3 * f32),
+              ('stack', 3 * f32), ('x + r', 3 * f32), ('/ (2 r)', 3 * f32), ('* 1', 3 * f32), ('+ 0', 3 * f32)]
+    if sphere:
+        per_op += [('u * 2', 3 * f32), ('- 1', 3 * f32), ('norm', f32), ('mag > 1', b8), ('1 / mag', f32), ('2 - 1 / mag', f32), ('v / mag', 3 * f32),
+                   ('(2 - 1 / mag) * (v / mag)', 3 * f32), ('where', 3 * f32), ('v / 4', 3 * f32), ('+ 0.5', 3 * f32)]
+    per_op += [('hash encoding (fp16)', 32 * f16), ('network output (fp16)', 16 * f16), ('raw0 + density_bias (fp16)', f16),
+               ('trunc_exp: .float()', f32), ('trunc_exp: exp', f32), ('negation', f32), ('level', f32)]
+    return {'fused': sum(b for _, b in per_op), 'fused_export': f32, 'fused_items': dict(per_op)}
+
+
+def main_nerf(args, dev, card):
+    res_list = [int(r) for r in args.res.split(',')]
+    for name in ('nerf-blender', 'nerf-colmap'):
+        if args.only not in name:
+            continue
+        model = build(name, dev, res_list[0])
+        b = level_bytes_per_point(name == 'nerf-colmap')
+        print(json.dumps(dict(workload=name, level_bytes_per_point={'fused (forward_level)': b['fused'], 'fused_export (lattice kernel)':
+                                                                    b['fused_export']}, forward_level_items=b['fused_items'])), flush=True)
+        for res in res_list:
+            model.geometry.config.isosurface['resolution'] = res
+            ways = [w for w in NERF_WAYS if w != 'default' or res <= DENSE_MAX]
+            runs = args.runs if res <= 512 else (min(args.runs, 2) if res <= 1024 else 1)
+            last = {w: run_nerf(model, w) for w in ways} if res <= DENSE_MAX else {w: (0.0, 0, None) for w in ways}   # warm-up
+            times = {w: [] for w in ways}
+            for _ in range(runs):
+                for w in ways:
+                    dt, peak, mesh = run_nerf(model, w)
+                    times[w].append(dt)
+                    last[w] = (dt, max(peak, last[w][1]), mesh)
+            for w in ways:
+                report(card, name, w, times[w], last[w][1], last[w][2], res)
+            ref = last['fused'][2]
+            for w in ways:
+                m = last[w][2]
+                same = torch.equal(m['v_pos'], ref['v_pos']) and torch.equal(m['t_pos_idx'], ref['t_pos_idx'])
+                print(json.dumps(dict(workload=name, resolution=res, path=w, mesh_bit_identical_to_fused=bool(same))), flush=True)
+            del last, ref
+            torch.cuda.empty_cache()
+        del model
+
+
 def report(card, label, path, times, peak, mesh, resolution):
     print(json.dumps(dict(workload=label, path=path, resolution=resolution, median_s=round(statistics.median(times), 4),
                           runs=[round(t, 4) for t in times], peak_mib=round(peak / 2 ** 20, 1), vertices=int(mesh['v_pos'].shape[0]),
@@ -88,10 +157,14 @@ def main():
     ap.add_argument('--runs', type=int, default=3)
     ap.add_argument('--only', default='', help='run only the workloads whose name contains this string')
     ap.add_argument('--no-large', action='store_true', help='skip the fused-only 1024^3 and 2048^3 runs')
+    ap.add_argument('--nerf', action='store_true', help='the NeRF density fields, three ways (see above)')
+    ap.add_argument('--res', default='256,512,1024,2048', help='--nerf: resolutions')
     args = ap.parse_args()
     dev = torch.device('cuda:0')
     card = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i', '0'],
                           capture_output=True, text=True).stdout.strip()
+    if args.nerf:
+        return main_nerf(args, dev, card)
     for name, res, levels in (('neus-blender', 512, None), ('neuralangelo-dtu-wmask', 512, 9), ('neuralangelo-dtu-wmask', 512, 16),
                               ('nerf-blender', 256, None)):
         if args.only not in name:
